@@ -191,15 +191,6 @@ class ClockSampler(threading.Thread):
         return {"sm_mhz": float(np.median(sm)), "sm_max_mhz": float(max(mx)), "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def measured_traffic(kernel):
-    """DRAM bytes per launch of a kernel from the committed `ncu --set full` capture (profiles/traffic.json), or None."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        return json.load(open(p)).get(kernel)
-    except Exception:
-        return None
-
-
 def hbm_peak():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
@@ -207,7 +198,7 @@ def hbm_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 # ======================================================================================================
@@ -328,6 +319,34 @@ def _file_barrier(cid, cfg, timeout_s=3600):
     return wait
 
 
+DUMP_NN_SAMPLE = 4096   # queries per edge whose match --dump-outputs writes (a fixed, seeded sample)
+
+
+def dump_outputs(out_dir, eng, poses, edges, world):
+    """What the timed path computed in its last step, as a caller of the engine receives it: the poses (float64 [M, 4, 4]), and for
+    the edges of a single-GPU run the weights (float64 [E]) and, on a fixed seeded sample of every edge's queries, the match index
+    and squared distance (float64 [E, DUMP_NN_SAMPLE]; -1 / 0 for an edge without queries).  Inputs are seeded: two builds given the
+    same arguments can be compared array by array."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "poses.npy"), np.asarray(poses, np.float64))
+    if world > 1:      # the per-edge results of a sharded run live on the ranks that own the edges
+        return
+    E = len(edges)
+    w = np.zeros(E); idx = np.full((E, DUMP_NN_SAMPLE), -1.0); d2 = np.zeros((E, DUMP_NN_SAMPLE))
+    rng = np.random.default_rng(0xD0)
+    for e, (s, _) in enumerate(edges):
+        w[e] = float(eng.get_edge(e, arrays=False)[1])
+        n = eng.n_pts[s]
+        pick = np.sort(rng.choice(n, size=min(n, DUMP_NN_SAMPLE), replace=False))
+        if s == 0:     # frame 0 is fixed: its edges are never searched
+            continue
+        i, d = eng.get_nn(e)
+        idx[e, :len(pick)] = i[pick]; d2[e, :len(pick)] = d[pick]
+    np.save(os.path.join(out_dir, "edge_weights.npy"), w)
+    np.save(os.path.join(out_dir, "nn_idx_sample.npy"), idx)
+    np.save(os.path.join(out_dir, "nn_d2_sample.npy"), d2)
+
+
 def run_ours(args, cfg):
     rank = int(os.environ.get("RANK", "0")); world = int(os.environ.get("WORLD_SIZE", "1")); local = int(os.environ.get("LOCAL_RANK", "0"))
     sc = load_scene(args.config, cfg, rank, world, _file_barrier(args.config, cfg) if (world > 1 and args.config != "real") else None)
@@ -445,6 +464,8 @@ def run_ours(args, cfg):
     wall_total = time.perf_counter() - t0
     st1 = eng.stats(); l1 = st1["kernel_launches"]
     final_poses = eng.get_poses()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, final_poses, edges, world)
     # e2e: same K rounds, poses cross the C ABI as host buffers every step
     barrier()
     t0 = time.perf_counter()
@@ -515,11 +536,11 @@ def run_ours(args, cfg):
         dominant = "knn" if share["knn"] >= share["lm_eval"] else "lm_eval"
         knn_name = "knn_kernel"      # the NN step of a round: knn_far_kernel (rounds 0-1), knn_kernel, or knn_cert_kernel + knn_todo_kernel (certified rounds)
         roof_knn = {"kernel": knn_name, "bound": "hbm", "achieved": knn_gbs, "peak": peak, "unit": "GB/s", "frac": knn_gbs / peak,
-                    "traffic": measured_traffic(knn_name) if world == 1 else None, "algorithmic_bytes_per_launch": knn_bytes,
+                    "algorithmic_bytes_per_launch": knn_bytes,
                     "avg_launch_ms": knn_ms, "peak_source": peak_src,
                     "frac_per_round": [round(44.0 * p["queries"] / (p["knn_ms"] * 1e-3) / 1e9 / peak, 4) for p in per]}
         roof_lm = {"kernel": "lm_eval_kernel", "bound": "hbm", "achieved": lm_gbs, "peak": peak, "unit": "GB/s", "frac": lm_gbs / peak,
-                   "traffic": measured_traffic("lm_eval_kernel") if world == 1 else None, "algorithmic_bytes_per_launch": lm_bytes,
+                   "algorithmic_bytes_per_launch": lm_bytes,
                    "avg_launch_ms": lm_eval_ms / max(1, evals), "peak_source": peak_src}
         pose_bytes = M * 16 * 8
         n_q = sum(n_pts[s] for s, _ in edges)
@@ -527,7 +548,7 @@ def run_ours(args, cfg):
                "warmup": max(3, args.warmup), "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
                "dtype": "f64", "data": "real scans (tests/golden/bunny18.npz)" if sc.get("real") else "synthetic",
                "config": {"workload": workload_name(args.config, cfg),
-                          "l2": "no flush: resident working set (clouds + trees + match arrays) = %.0f MB > 126 MB L2" %
+                          "l2": "no flush: resident working set (clouds + trees + match arrays) = %.0f MB > 50 MB L2" %
                                 ((sum(n_pts) * 48 + n_q * 12) / 1e6),
                           "parallelism": f"edges (frame -> neighbour query sets) sharded over {world} GPU(s), one process per GPU",
                           "timing_passes": "value / e2e: K calls between barriers, nothing else in the loop; per-round and per-kernel figures: the same K rounds repeated with events + sync + stats per round (same final poses, checked)",
@@ -616,6 +637,7 @@ def main():
     ap.add_argument("--single-rounds", type=int, default=2, help="reference arm: rounds of the single-thread leg (0: skip)")
     ap.add_argument("--check-cpu", action="store_true", help="replay every round on the CPU from the GPU's poses and compare counts / poses")
     ap.add_argument("--flags", type=int, default=0, help="MVICP_FLAG_* bits for the engine (A/B measurements)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the timed steps computed in their last step to DIR/*.npy")
     args = ap.parse_args()
     cfg = CONFIGS[args.config]
     if args.impl == "reference":

@@ -1,4 +1,4 @@
-/* mvicp.h -- C ABI of the B200-native multiview LM-ICP engine (libmvicp.so).
+/* mvicp.h -- C ABI of the H100-native multiview LM-ICP engine (libmvicp.so).
  *
  * The reference (adrelino/mv-lm-icp) has no FFI layer: its hot path is a set of C++ signatures on
  * Eigen types called from two drivers.  Each entry point below names the reference interface it

@@ -1,4 +1,4 @@
-"""mv_lm_icp_b200 -- B200-native multiview LM-ICP engine (hot path of adrelino/mv-lm-icp).
+"""mv_lm_icp_b200 -- H100-native multiview LM-ICP engine (hot path of adrelino/mv-lm-icp).
 
 The product is the C-ABI library libmvicp.so (include/mvicp.h, csrc/); this package is its Python host mirror:
 `Engine` wraps a context, `Frame` / `ICP_Ceres`-style helpers follow the reference's names (include/frame.h,

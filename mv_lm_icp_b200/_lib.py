@@ -51,7 +51,7 @@ EXPORTS = ["mvicp_default_lm_options", "mvicp_last_error", "mvicp_create", "mvic
 
 
 def build(force=False):
-    """Compile libmvicp.so for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile libmvicp.so for sm_90a (nvcc cross-compiles without a GPU)."""
     srcs = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(_HERE, "..", "include", "mvicp.h")]
     stale = force or not os.path.exists(LIB_PATH) or any(os.path.getmtime(s) > os.path.getmtime(LIB_PATH) for s in srcs)
     if stale:

@@ -5,9 +5,9 @@
 // to q, e = |q - s*|.  A point p of leaf T with |p - q| <= r satisfies boxdist(S, T) <= |s* - p| <= e + r.  So if e + r <= R_S
 // every point within r of q lies in S or in a leaf of adj(S): a seeded query whose start leaf gives it a reach e + r <= R_S
 // needs no tree walk at all -- it tests the listed leaves' boxes and scans those that can still hold a closer point (knn.cuh).
-// Measured motivation (config 3, converged round): the walk up 15 ancestor levels and the divergent descents that follow
-// were 80 % of the NN kernel's instructions, to find on average 0.6 neighbouring leaves per query; with R_S = 0.6 diagonals
-// 95 % of the queries are inside their leaf's reach and the lists hold 9-10 leaves (tools/sim_search.cpp).
+// Motivation (config 3, converged round): the walk up 15 ancestor levels and the divergent descents that follow find on
+// average 0.6 neighbouring leaves per query; with R_S = 0.6 diagonals 95 % of the queries are inside their leaf's reach and
+// the lists hold 9-10 leaves (host model, tools/sim_search.cpp).
 // Boxes are the stored fp32 boxes (rounded outward): distances between them can only be SMALLER than between the true boxes,
 // so a list can only gain members by rounding, never lose one.
 #pragma once

@@ -4,11 +4,9 @@
 // A depth scan is a tilted, locally flat sheet: its axis-aligned boxes are as thick as the tilt makes them, and a query
 // that is still millimetres off the surface has to open every box within sqrt(height x thickness) of its foot point.  Nodes
 // of up to 64 points therefore get the box of their principal axes when that is clearly smaller (volume ratio < 0.5), all
-// others keep the coordinate axes (KD siblings stay disjoint near the root).  Measured on a B200 (profiles/r2, config 3):
-// round 0 11.1 -> 9.0 ms, round 1 6.6 -> 5.9 ms; from the second seeded round on the 32-byte AABB nodes of knn.cuh win
-// (64-byte nodes cost more than the tighter boxes save once the seeds are good), hence a second node array and the switch
-// in mvicp_correspond.  MVICP_FLAG_NO_OBB builds no such array: every round then runs knn_kernel.  (Trying the per-leaf
-// neighbour lists of knn.cuh first, for the seeds that are still good, measured no gain here: 3.52 -> 3.65 ms in round 1.)
+// others keep the coordinate axes (KD siblings stay disjoint near the root).  From the second seeded round on the 32-byte
+// AABB nodes of knn.cuh win (64-byte nodes cost more than the tighter boxes save once the seeds are good), hence a second
+// node array and the switch in mvicp_correspond.  MVICP_FLAG_NO_OBB builds no such array: every round then runs knn_kernel.
 #pragma once
 #include "knn.cuh"
 

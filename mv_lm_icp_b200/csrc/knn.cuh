@@ -113,7 +113,7 @@ template <class Q> __device__ __forceinline__ void nn_pruned(Q& s, float lb) {
   if constexpr (nn_track<Q>::value) s.lbmin = fminf(s.lbmin, lb);
 }
 // (Pruning boxes and planes against a slightly larger bound while a certificate is written -- so that a box just outside the exact
-// bound does not leave a margin of nothing -- was measured: kept queries 95.5 -> 96.5 %, but every search dearer: 531 -> 515 iter/s.)
+// bound does not leave a margin of nothing -- keeps a few more queries but makes every search dearer.)
 // r <= sqrt(b)
 __device__ __forceinline__ float sqrt_lower(float b) {
 #ifdef __CUDA_ARCH__
@@ -431,8 +431,8 @@ knn_kernel(const FrameDev* __restrict__ frames, const EdgeDev* __restrict__ edge
 // ---- certified rounds: two launches instead of knn_kernel -------------------------------------------------------------------------
 // knn_cert_kernel streams over all queries: a query that is still within half its margin of the certified position keeps its match
 // and only recomputes the distance (knn_one, MODE 1); the others are appended to a device-wide list.  knn_todo_kernel then searches
-// and re-certifies the listed queries with every lane busy.  (Searching them inside the first kernel -- even compacted per CTA --
-// measured SLOWER than searching everything: a CTA's finished warps hold their slots while one warp walks the tree, 0.65 vs 0.55 ms.)
+// and re-certifies the listed queries with every lane busy.  (Searching them inside the first kernel, even compacted per CTA, is
+// slower than searching everything: a CTA's finished warps hold their slots while one warp walks the tree.)
 struct CertTodo { int2* list; unsigned int* n; };     // {edge, position in the src frame's tree order}
 
 template <bool F32>

@@ -271,11 +271,11 @@ static int set_frames_device(mvicp_ctx* c, int M, const double* const* pts, cons
     const size_t bytes = sizeof(double) * 3 * (size_t)n_pts[f];
     err = cudaMalloc(&d_xyz[f], bytes);
     if (err == cudaSuccess) err = cudaMemcpyAsync(d_xyz[f], pts[f], bytes, cudaMemcpyHostToDevice, c->stream);
-    if (err == cudaSuccess) kd_scan_kernel<<<2 * 148, 256, 0, c->stream>>>(d_xyz[f], 3ll * n_pts[f], d_flags + 4 * f);
+    if (err == cudaSuccess) kd_scan_kernel<<<2 * NUM_SMS, 256, 0, c->stream>>>(d_xyz[f], 3ll * n_pts[f], d_flags + 4 * f);
     if (err == cudaSuccess && nor && nor[f]) {
       err = cudaMalloc(&d_nor[f], bytes);
       if (err == cudaSuccess) err = cudaMemcpyAsync(d_nor[f], nor[f], bytes, cudaMemcpyHostToDevice, c->stream);
-      if (err == cudaSuccess) kd_scan_kernel<<<2 * 148, 256, 0, c->stream>>>(d_nor[f], 3ll * n_pts[f], d_flags + 4 * f + 2);
+      if (err == cudaSuccess) kd_scan_kernel<<<2 * NUM_SMS, 256, 0, c->stream>>>(d_nor[f], 3ll * n_pts[f], d_flags + 4 * f + 2);
     }
     c->stats.kernel_launches += (nor && nor[f]) ? 2 : 1;
   }
@@ -528,14 +528,14 @@ static int layout_work(mvicp_ctx* c) {
     if (ed.owned) owned_slots += ed.n_src;
   }
   c->total_slots = off;
-  // LM streaming tile: long enough to amortise the 28-value block reduction, short enough to fill 148 SMs.  Its length fixes how
+  // LM streaming tile: long enough to amortise the 28-value block reduction, short enough to fill the SMs.  Its length fixes how
   // an edge's sum is associated (per-tile partials, added in tile order), so it must not depend on how many ranks share the
   // work: it is chosen from ALL active slots, and a sharded run's poses stay bit-identical to the single-GPU run's
   // (bench.py checks that in every multi-GPU run; round 1 chose it from the rank's own share and was not).
   int64_t active_slots = 0;
   for (int e = 0; e < E; ++e) if (c->edge_owner[e] >= 0) active_slots += c->h_edges[e].n_src;
   int tl = 8192;
-  while (tl > 1024 && active_slots / tl < 8 * 148) tl >>= 1;
+  while (tl > 1024 && active_slots / tl < 8 * NUM_SMS) tl >>= 1;
   c->eval_tile_len = tl;
   (void)owned_slots;
   std::vector<Tile> kt, et; std::vector<int32_t> etb(E + 1, 0);
@@ -666,11 +666,8 @@ template <bool F32> static int launch_correspond(mvicp_ctx* c, float thresh) {
   const bool ww = !(c->flags & MVICP_FLAG_STEP_LOOP);
   if (c->n_knn_tiles) {
     // Far rounds search the oriented-box node array (far.cuh): a round without seeds, and the first round that has them (its
-    // seeds were found before the first LM solve moved the clouds by centimetres).  Measured on config 3 (profiles/r2): round 0
-    // 11.1 -> 9.0 ms, round 1 6.6 -> 5.9 ms; from the second seeded round on the 32-byte AABB nodes win (4.57 vs 4.96 ms).
-    // Poses set from outside since the last solve count as a fresh start.
-    // (Keeping later seeded rounds on the oriented boxes while the solves still take >= 4 LM iterations: rounds 2-3 2.30 -> 2.98,
-    // 1.51 -> 2.11 ms, profiles/r2/s10_*.)
+    // seeds were found before the first LM solve moved the clouds by centimetres); from the second seeded round on the 64-byte
+    // oriented boxes cost more than their tighter fit saves.  Poses set from outside since the last solve count as a fresh start.
     if (!seed || c->last_lm_iters == (1 << 20)) c->seeded_rounds = 0;
     far = c->obb_ready && (!seed || c->seeded_rounds < 1);
     if (seed) ++c->seeded_rounds;
@@ -696,7 +693,7 @@ template <bool F32> static int launch_correspond(mvicp_ctx* c, float thresh) {
     else if (cert == 2) {
       const CertTodo todo = {c->d_todo.as<int2>(), c->d_todo_n.as<unsigned int>()};
       knn_cert_kernel<F32><<<c->n_knn_tiles, KNN_TILE, 0, c->stream>>>(MV_KNN_ARGS, MV_KNN_TAIL, c->d_cert_cnt.as<unsigned long long>(), todo);
-      knn_todo_kernel<F32><<<148 * 5, KNN_TILE, 0, c->stream>>>(c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_xf.as<EdgeXf>(),
+      knn_todo_kernel<F32><<<NUM_SMS * 5, KNN_TILE, 0, c->stream>>>(c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_xf.as<EdgeXf>(),
           c->d_corr.as<int32_t>(), c->d_d2.as<double>(), c->d_corr.as<int32_t>(), d2max, MV_KNN_TAIL, todo);
       c->stats.kernel_launches += 1;
     }
@@ -1114,7 +1111,7 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
   }
   // sharded runs: every rank holds bit-identical poses (the same lm_step_kernel ran on bit-identical pair matrices), so
   // no pose exchange is needed; the NCCL-only mode still all-gathers the owners' copies (6-dof poses per outer iteration,
-  // as the north-star words it) -- it costs ~0.1 ms of small copies at 8 ranks and changes nothing.
+  // as the north-star words it) -- a few small copies that change nothing.
   if (c->comm && c->world > 1 && !use_p2p) {
     const int chunk = (M + c->world - 1) / c->world;
     RET(c->d_posegather.reserve(sizeof(double) * 16 * (size_t)chunk * c->world * 2));
@@ -1212,7 +1209,7 @@ int mvicp_pairwise_closed(const mvicp_config* cfg, int32_t cost, const double* s
   CU(cudaSetDevice(dev));
   cudaStream_t st = cfg && cfg->stream ? (cudaStream_t)cfg->stream : nullptr;
   const size_t bytes = sizeof(double) * 3 * (size_t)n;
-  const int grid = (int)std::min<int64_t>(2 * 148, (n + CLOSED_THREADS - 1) / CLOSED_THREADS);
+  const int grid = (int)std::min<int64_t>(2 * NUM_SMS, (n + CLOSED_THREADS - 1) / CLOSED_THREADS);
   double *d_src = nullptr, *d_dst = nullptr, *d_nor = nullptr, *d_part = nullptr, *d_aux = nullptr;
   std::vector<double> part((size_t)grid * CLOSED_MAXV);
   auto cleanup = [&]() { cudaFree(d_src); cudaFree(d_dst); cudaFree(d_nor); cudaFree(d_part); cudaFree(d_aux); };

@@ -20,6 +20,8 @@ bunny18.npz      the reference's DEFAULT multiview workload (main_multiview.cpp:
                  (frame 0 = GT, the others addNoise(GT, 0.02, 0.01), common.h:38-67; the reference's default-seeded mt19937 stream
                  is not reproduced -- same noise model, numpy seed 0xB18).  Used by `bench.py --config real` and tests/test_gpu_real18.py.
 sophus_vectors.npz  the SE3 group elements / tangents of ext/sophus-ceres/test/core/test_se3.cpp:40-82 (values only).
+ref_nanoflann.npz   answers of the reference's nanoflann for tests/test_oracle_corr.py (a synthetic edge as sha256, k-NN on bunny_pair).
+functor_pin.npz     outputs of the reference's cost-functor text on the first inputs of tests/test_oracle_functor_pin.py.
 """
 import os
 import sys
@@ -103,6 +105,48 @@ def lm_golden():
     np.savez_compressed(os.path.join(OUT, "lm_golden.npz"), **out)
 
 
+def ref_nanoflann():
+    """Answers of the reference's nanoflann for tests/test_oracle_corr.py: sha256 of the 1-NN indices / squared distances of the
+    synthetic edge of test_restatement_equals_reference_nanoflann, and the 10-NN of every 53rd point of bunny_pair's pts0."""
+    import hashlib
+    sys.path.insert(0, os.path.dirname(OUT))
+    from helpers import scene
+    sha = lambda a: hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+    sc = scene(3, 20000, 32)
+    out = {}
+    for k, poses in enumerate((sc["poses_init"], sc["poses_gt"])):
+        idx, d2 = O.KdIndex(sc["pts"][0], "ref").closest_points(sc["pts"][1], poses[1], poses[0], threads=4)
+        out[f"synth_idx_sha{k}"] = np.array(sha(idx)); out[f"synth_d2_sha{k}"] = np.array(sha(d2))
+    pts = np.load(os.path.join(OUT, "bunny_pair.npz"))["pts0"]
+    rf = O.KdIndex(pts, "ref")
+    nn = [O.knn(rf, pts[i], 10) for i in range(0, len(pts), 53)]
+    out["bunny_knn_idx"] = np.stack([a for a, _ in nn]); out["bunny_knn_d2"] = np.stack([b for _, b in nn])
+    np.savez_compressed(os.path.join(OUT, "ref_nanoflann.npz"), **out)
+
+
+def functor_pin(n_global=32, n_pairwise=16, n_quat=100):
+    """Outputs of the reference's functor text (oracle/_ref/libref_functors.so) on the first inputs of every case of
+    tests/test_oracle_functor_pin.py."""
+    import ctypes as C
+    sys.path.insert(0, os.path.dirname(OUT))
+    import test_oracle_functor_pin as T
+    out = {}
+    for param in (0, 1, 2):
+        for plane in (0, 1):
+            res = [O.functor_eval(param, plane, *a, "ref") for a, _ in zip(T._global_cases(param, plane), range(n_global))]
+            out[f"global_{param}{plane}_r"] = np.stack([r for r, _ in res]); out[f"global_{param}{plane}_j"] = np.stack([j for _, j in res])
+            res = [O.functor_eval_pairwise_ref(param, plane, *a) for a, _ in zip(T._pairwise_cases(param, plane), range(n_pairwise))]
+            out[f"pairwise_{param}{plane}_r"] = np.stack([r for r, _ in res]); out[f"pairwise_{param}{plane}_j"] = np.stack([j for _, j in res])
+    lib = O.ref_functors()
+    P = lambda a: a.ctypes.data_as(C.POINTER(C.c_double))
+    qr, qj = [], []
+    for (x, d), _ in zip(T._quat_cases(), range(n_quat)):
+        o = np.zeros(4); lib.ref_quat_plus(P(x), P(d), P(o)); j = np.zeros(12); lib.ref_quat_jacobian(P(x), P(j))
+        qr.append(o); qj.append(j)
+    out["quat_r"] = np.stack(qr); out["quat_j"] = np.stack(qj)
+    np.savez_compressed(os.path.join(OUT, "functor_pin.npz"), **out)
+
+
 def sophus_vectors():
     # ext/sophus-ceres/test/core/test_se3.cpp:40-65: SE3(SO3::exp(w), t) ; :67-82 tangents (upsilon, omega)
     pi = np.pi
@@ -118,6 +162,6 @@ def sophus_vectors():
 
 if __name__ == "__main__":
     only = sys.argv[1:]
-    for fn in (bunny_pair, dino_pair, lm_golden, sophus_vectors, bunny18):
+    for fn in (bunny_pair, dino_pair, lm_golden, sophus_vectors, bunny18, ref_nanoflann, functor_pin):
         if not only or fn.__name__ in only:
             fn()

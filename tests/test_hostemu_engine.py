@@ -212,7 +212,7 @@ def test_closed_form_pairwise(emu, oracle):
 def test_every_kernel_family_under_address_sanitizer(tmp_path):
     """tools/sanitize_run.py (every kernel family, both storage modes, general path, 40 views, experimental schedules) + the
     closed forms on an AddressSanitizer build of the emulated engine: device buffers are heap blocks there, so an out-of-bounds
-    access by a kernel aborts the run (the CPU counterpart of profiles/r1_sanitizer.txt's memcheck)."""
+    access by a kernel aborts the run (the CPU counterpart of compute-sanitizer's memcheck)."""
     import subprocess
     import build_hostemu
     so = build_hostemu.build(asan=True)

@@ -1,7 +1,9 @@
-"""Pins the oracle's correspondence restatement (oracle_icp.cpp) against the reference's own nanoflann compiled from
-/root/reference (oracle/_ref), against brute force, and against the committed golden vectors."""
+"""Pins the oracle's correspondence restatement (oracle_icp.cpp) against the reference's own nanoflann (oracle/_ref, built
+where the reference tree is present, and its answers stored under tests/golden), against brute force, and against the committed
+golden vectors."""
+import hashlib
+
 import numpy as np
-import pytest
 
 from helpers import scene
 from mv_lm_icp_b200 import synth
@@ -20,13 +22,21 @@ def test_kd_restatement_equals_brute_force(oracle):
         assert np.array_equal(a[0], b[0]) and np.array_equal(a[1].view(np.uint64), b[1].view(np.uint64))
 
 
-def test_restatement_equals_reference_nanoflann(oracle):
-    if oracle.ref_lib() is None:
-        pytest.skip("oracle/_ref not built (no /root/reference and no prebuilt .so)")
+def _sha(a):
+    return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()
+
+
+def test_restatement_equals_reference_nanoflann(oracle, golden_dir):
+    """Against the reference's nanoflann itself when oracle/_ref was built, and always against the sha256 of its answers
+    (tests/golden/ref_nanoflann.npz, make_golden.py:ref_nanoflann)."""
+    g = np.load(f"{golden_dir}/ref_nanoflann.npz")
     sc, (s, d) = _edge_inputs(20000, 32)
     ties = 0
-    for poses in (sc["poses_init"], sc["poses_gt"]):
+    for k, poses in enumerate((sc["poses_init"], sc["poses_gt"])):
         a = oracle.KdIndex(sc["pts"][d], "kd").closest_points(sc["pts"][s], poses[s], poses[d], threads=4)
+        assert _sha(a[0]) == g[f"synth_idx_sha{k}"] and _sha(a[1]) == g[f"synth_d2_sha{k}"], k
+        if oracle.ref_lib() is None:
+            continue
         r = oracle.KdIndex(sc["pts"][d], "ref").closest_points(sc["pts"][s], poses[s], poses[d], threads=4)
         assert np.array_equal(a[1].view(np.uint64), r[1].view(np.uint64))    # minimal squared distance: bit-exact
         ties += int((a[0] != r[0]).sum())                                     # index may differ only on exact ties
@@ -92,14 +102,13 @@ def test_knn_restatement_equals_reference_nanoflann(oracle, golden_dir):
     """Frame::getNeighbours (frame.cpp:208-242): the oracle's k-NN against the reference's nanoflann knnSearch on the
     reference's own scan.  Squared distances must agree bit for bit; indices may differ only inside groups of exactly
     equal distance (the scan's coordinates are quantised, so such ties exist; nanoflann orders them by traversal)."""
-    if oracle.ref_lib() is None:
-        pytest.skip("oracle/_ref not built")
     g = np.load(f"{golden_dir}/bunny_pair.npz")
+    gk = np.load(f"{golden_dir}/ref_nanoflann.npz")     # the reference's answers, for when oracle/_ref was not built
     pts = g["pts0"]
-    kd = oracle.KdIndex(pts, "kd"); rf = oracle.KdIndex(pts, "ref")
+    kd = oracle.KdIndex(pts, "kd"); rf = oracle.KdIndex(pts, "ref") if oracle.ref_lib() is not None else None
     differing = 0
-    for i in range(0, len(pts), 53):
-        a = oracle.knn(kd, pts[i], 10); b = oracle.knn(rf, pts[i], 10)
+    for k, i in enumerate(range(0, len(pts), 53)):
+        a = oracle.knn(kd, pts[i], 10); b = oracle.knn(rf, pts[i], 10) if rf is not None else (gk["bunny_knn_idx"][k], gk["bunny_knn_d2"][k])
         assert np.array_equal(a[1].view(np.uint64), b[1].view(np.uint64))
         assert a[0][0] == i == b[0][0] and a[1][0] == 0.0            # the point itself comes first
         if not np.array_equal(a[0], b[0]):
