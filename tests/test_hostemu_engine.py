@@ -105,6 +105,12 @@ def test_normals(emu, oracle, golden_dir):
         T.test_normals_real_scan_and_lm_uses_them(oracle, golden_dir)
 
 
+def test_knn_self_and_normals_at_every_k(emu):
+    import test_gpu_fuzz as T
+    T.test_knn_self_every_k()
+    T.test_normals_every_k()
+
+
 def test_headless_driver_on_the_emulated_engine(emu, tmp_path):
     """apps/multiview_main.cpp linked against the emulated library: the reference's file formats, flags and loop end to end,
     bit-identical to the Python mirror of the same loop (what tests/test_app_multiview.py checks on the GPU)."""
