@@ -7,6 +7,8 @@
 // others keep the coordinate axes (KD siblings stay disjoint near the root).  From the second seeded round on the 32-byte
 // AABB nodes of knn.cuh win (64-byte nodes cost more than the tighter boxes save once the seeds are good), hence a second
 // node array and the switch in mvicp_correspond.  MVICP_FLAG_NO_OBB builds no such array: every round then runs knn_kernel.
+// Above the PCA level (nodes of more than OBB_PCA_LEAVES leaves) an oriented box is always the box of the coordinate axes, and
+// the 32-byte fp32 AABB of knn.cuh bounds the same points as tightly (up to rounding) in half the bytes: the search reads it there.
 #pragma once
 #include "knn.cuh"
 
@@ -28,10 +30,12 @@ __device__ __forceinline__ float obb_lb32(const ObbNode* __restrict__ nodes, int
   return fmaf(g2, g2, fmaf(g1, g1, g0 * g0));
 }
 
-// nn_search of knn.cuh with the oriented lower bound (the split-plane pre-filter and the stale-seed rule are unchanged)
+// nn_search of knn.cuh with the hybrid lower bound (the split-plane pre-filter and the stale-seed rule are unchanged)
 template <bool F32, bool WW>
 __device__ __forceinline__ void nn_search_obb(const FrameDev& fd, const ObbNode* __restrict__ ob, NNQuery& s, int start_leaf) {
   const int L = fd.n_leaf_pad;
+  const int pca_first = L / OBB_PCA_LEAVES;   // first node that may hold principal axes
+  const auto lb_of = [&](int nd) { return nd < pca_first ? box_lb32(fd.boxes, nd, s) : obb_lb32(ob, nd, s); };
   int leaf_node = -1;
   if (start_leaf >= 0) {
     leaf_node = L + start_leaf;
@@ -46,7 +50,7 @@ __device__ __forceinline__ void nn_search_obb(const FrameDev& fd, const ObbNode*
     int node = 1;
     while (node < L) {
       const int c0 = 2 * node;
-      const float l0 = obb_lb32(ob, c0, s), l1 = obb_lb32(ob, c0 + 1, s);
+      const float l0 = lb_of(c0), l1 = lb_of(c0 + 1);
       node = (l1 < l0) ? c0 + 1 : c0;
     }
     if (node != leaf_node) {
@@ -63,10 +67,10 @@ __device__ __forceinline__ void nn_search_obb(const FrameDev& fd, const ObbNode*
     const float qa = axis == 0 ? s.fx : (axis == 1 ? s.fy : s.fz);
     const float dpl = (sib & 1) ? face - qa : qa - face;
     if (dpl > 0.f && dpl * dpl > s.bound32) continue;
-    const float lb = obb_lb32(ob, sib, s);
+    const float lb = lb_of(sib);
     if (lb <= s.bound32) { stk_n[sp] = sib; stk_lb[sp] = lb; ++sp; }
   }
-  nn_drain<F32, WW, NNQuery>(fd, s, stk_n, stk_lb, sp, [&](int nd) { return obb_lb32(ob, nd, s); });
+  nn_drain<F32, WW, NNQuery>(fd, s, stk_n, stk_lb, sp, lb_of);
 }
 
 template <bool F32, bool WW>

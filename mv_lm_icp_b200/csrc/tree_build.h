@@ -103,12 +103,11 @@ static void build_frame(const double* pts, int64_t n, HostFrameBuild& out) {
 
 
 // ---- hybrid oriented boxes for the far-round search (far.cuh, MVICP_FLAG_OBB_FAR) ---------------------------------------
-// Per node either the box of the coordinate axes or -- for nodes of at most OBB_PCA_MAX_LEAVES leaves whose principal-axes
+// Per node either the box of the coordinate axes or -- for nodes of at most OBB_PCA_LEAVES leaves whose principal-axes
 // box is clearly smaller -- the box of the principal axes of its points.  The extents are taken in fp64 against the STORED
 // fp32 centre and axes, so the containment the kernel relies on is exact for them; (1 + 1e-6) covers |A x| <= (1 + 1e-6)|x|
 // for axes that are orthonormal to 2e-7 (else the node keeps the coordinate axes).
 struct ObbHost { float c[3]; float e0; float a0[3]; float e1; float a1[3]; float e2; float a2[3]; float pad; };
-static const int OBB_PCA_MAX_LEAVES = 8;
 static const double OBB_PCA_RATIO = 0.5;
 
 static void build_obb(const double* pts, int64_t n, const HostFrameBuild& hb, std::vector<ObbHost>& out) {
@@ -143,7 +142,7 @@ static void build_obb(const double* pts, int64_t n, const HostFrameBuild& hb, st
                         {0, 0, mm.ss[5] / mm.n - mean[2] * mean[2]}};
       C[1][0] = C[0][1]; C[2][0] = C[0][2]; C[2][1] = C[1][2];
       double V[3][3] = {{1, 0, 0}, {0, 1, 0}, {0, 0, 1}};
-      if (mm.n >= 3 && per <= OBB_PCA_MAX_LEAVES) {   // cyclic Jacobi, symmetric 3x3
+      if (mm.n >= 3 && per <= OBB_PCA_LEAVES) {   // cyclic Jacobi, symmetric 3x3
         for (int sweep = 0; sweep < 12; ++sweep) {
           if (std::fabs(C[0][1]) + std::fabs(C[0][2]) + std::fabs(C[1][2]) < 1e-30) break;
           for (int p = 0; p < 2; ++p)
@@ -166,7 +165,7 @@ static void build_obb(const double* pts, int64_t n, const HostFrameBuild& hb, st
         float A[3][3];
         for (int a = 0; a < 3; ++a) for (int k = 0; k < 3; ++k) A[a][k] = cand == 0 ? (a == k ? 1.f : 0.f) : (float)V[k][a];
         if (cand == 1) {
-          if (per > OBB_PCA_MAX_LEAVES) break;
+          if (per > OBB_PCA_LEAVES) break;
           bool ortho = true;
           for (int a = 0; a < 3; ++a)
             for (int k = a; k < 3; ++k) {

@@ -214,7 +214,6 @@ __global__ void kd_adj_kernel(const Box* __restrict__ boxes, int L, int n_leaf, 
 
 // hybrid oriented boxes (tree_build.h:build_obb, same rules): per node the box of the coordinate axes, or -- nodes of at most
 // OBB_PCA_LEAVES leaves whose principal-axes box is clearly smaller -- the box of the principal axes of its points
-constexpr int OBB_PCA_LEAVES = 8;
 __global__ void kd_obb_kernel(const double* __restrict__ xyz, const int* __restrict__ order, KdGeom g, const double* __restrict__ dbox,
                               const KdMom* __restrict__ mom, ObbNode* __restrict__ out) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -15,6 +15,7 @@
 namespace mv {
 
 constexpr int LEAF = 8;          // points per BVH leaf
+constexpr int OBB_PCA_LEAVES = 8;   // far-round oriented boxes: only nodes of at most this many leaves may take principal axes (far.cuh)
 constexpr int NUM_SMS = 132;     // H100 SXM: sizes the grid-stride launches and the LM streaming tile (mvicp.cu)
 constexpr int KNN_TILE = 256;    // queries per CTA of the NN kernel
 constexpr int EVAL_TILE = 2048;  // correspondence slots per CTA of the LM streaming kernel
