@@ -74,9 +74,10 @@ def test_pipeline_round_matches_oracle(oracle):
 
 @pytest.mark.parametrize("n_views", [29, 40])
 def test_many_views_factor_in_global_memory(oracle, n_views):
-    """The reference's default is --limit=40 frames (main_multiview.cpp:34): 6 x 39 = 234 unknowns, whose Cholesky factor no
-    longer fits the 227 KB of shared memory (n <= 166), so lm_step_kernel keeps it in global memory; 29 views = 168 is the
-    first size on that path.  Same parity bar as the small cases, two consecutive rounds."""
+    """The reference's default is --limit=40 frames (main_multiview.cpp:34): 6 x 39 = 234 unknowns.  lm_step_kernel stores the
+    factor row profile by row profile (skyline), and a ring's rows span two or three pose blocks, so these factors need 17 and
+    24 KB and stay in shared memory; only wide row profiles leave it (tests/test_gpu_lm_graphs.py::
+    test_wide_graph_factor_in_global_memory).  Same parity bar as the small cases, two consecutive rounds."""
     sc = scene(n_views, 1500, 41)
     edges = synth.ring_edges(n_views, 2)
     eng = Engine(); eng.set_frames(sc["pts"], sc["nor"]); eng.set_graph(edges)

@@ -98,6 +98,43 @@ def test_lm_many_views_global_factor(emu, oracle, n_views):
     T.test_many_views_factor_in_global_memory(oracle, n_views)
 
 
+def test_lm_storage_modes(emu, oracle):
+    """Every storage mode on both LM paths; the second pass runs SE3 only."""
+    import test_gpu_lm_graphs as T
+    for mode in T.MODES:
+        for path in ("unit", "general"):
+            for param in (T.PARAMS if emu.order == "ascending" else [T.PARAM_SE3]):
+                if not (path == "general" and param == T.PARAM_AA):
+                    T.test_storage_modes_match_oracle(oracle, mode, path, param)
+
+
+def test_lm_graphs_and_fixed_sets(emu, oracle):
+    import test_gpu_lm_graphs as T
+    for name in T.TOPOLOGIES:
+        T.test_graph_topologies_match_oracle(oracle, name)
+    for fixed in T.FIXED_SETS:
+        T.test_fixed_sets_match_oracle(oracle, fixed)
+    T.test_all_frames_fixed_leaves_poses_unchanged(oracle)
+    T.test_switching_fixed_sets_between_solves(oracle)
+    T.test_free_frame_without_residuals_counts_in_x_norm(oracle)
+
+
+@pytest.mark.parametrize("n_views,over", [(36, False), (48, True)])
+def test_lm_wide_graph(emu, oracle, n_views, over):
+    import test_gpu_lm_graphs as T
+    _first_pass_only(emu)
+    T.test_wide_graph_factor_in_global_memory(oracle, n_views, over)
+
+
+def test_lm_tile_boundaries(emu, oracle):
+    """The 1024-slot tile in both passes; the 2048-slot tile (2.2 M active slots) in the first."""
+    import test_gpu_lm_graphs as T
+    T.test_zero_inlier_edge_with_zero_weight_adds_nothing(oracle)
+    T.test_tile_boundaries_cost_readout(oracle, 1024)
+    if emu.order == "ascending":
+        T.check_tile_readout(oracle, 2048, params=[T.PARAM_SE3])
+
+
 def test_normals(emu, oracle, golden_dir):
     import test_gpu_normals as T
     T.test_normals_match_oracle_synthetic(oracle)
