@@ -145,6 +145,42 @@ void pairwise(int param, bool pointToPlane, const std::vector<Vec3>& src, const 
                        nor ? (*nor)[0].data() : nullptr, (int64_t)src.size(), nullptr, pose16_out, nullptr));
 }
 
+// ICP_G2O::g2oOptimizer (include/icp-g2o.h:14, icp-g2o.cpp:149-303): the g2o backend on the same session; frame 0 becomes fixed.
+// chi2 (nullable) receives chi2 before the first optimize() call and after every call (what icp-g2o.cpp:264,283 print).
+template <class FrameT>
+mvicp_g2o_summary g2oOptimizer(Session<FrameT>& s, std::vector<std::shared_ptr<FrameT>>& frames, bool pointToPlane,
+                               std::vector<double>* chi2 = nullptr) {
+  s.bind(frames);
+  frames[0]->fixed = true;   // icp-g2o.cpp:182-186
+  if (!s.corr_valid) {       // caller filled OutgoingEdge::correspondances itself: hand them over
+    s.push_graph(); s.push_poses();
+    int32_t e = 0;
+    for (auto& f : frames)
+      for (auto& ne : f->neighbours) {
+        std::vector<int32_t> a, b;
+        for (auto& c : ne.correspondances) { a.push_back(c.first); b.push_back(c.second); }
+        check(mvicp_set_edge(s.ctx, e++, a.data(), b.data(), (int64_t)a.size(), ne.weight));
+      }
+  }
+  mvicp_g2o_summary sum{};
+  mvicp_g2o_options opt; mvicp_default_g2o_options(&opt);
+  std::vector<double> chi((size_t)opt.max_calls + 1, 0.0);
+  check(mvicp_optimize_g2o(s.ctx, pointToPlane ? MVICP_COST_P2PLANE : MVICP_COST_P2P, &opt, &sum, chi.data()));
+  if (chi2) chi2->assign(chi.begin(), chi.begin() + sum.calls + 1);
+  s.pull_poses();
+  s.corr_valid = false;
+  return sum;
+}
+
+// ICP_G2O::pointToPoint / pointToPlane (include/icp-g2o.h:10-11, icp-g2o.cpp:26-147): the src -> dst transform as 16 doubles.
+template <class Vec3>
+void pairwiseG2O(bool pointToPlane, const std::vector<Vec3>& src, const std::vector<Vec3>& dst, const std::vector<Vec3>* nor,
+                 double pose16_out[16]) {
+  mvicp_config cfg{0, 0, nullptr};
+  check(mvicp_pairwise_g2o(&cfg, pointToPlane ? MVICP_COST_P2PLANE : MVICP_COST_P2P, src[0].data(), dst[0].data(),
+                           nor ? (*nor)[0].data() : nullptr, (int64_t)src.size(), nullptr, pose16_out, nullptr));
+}
+
 // ICP_Closedform::pointToPoint / pointToPlane (include/icp-closedform.h; icp-closedform.cpp:9-54).
 template <class Vec3>
 void closedForm(bool pointToPlane, const std::vector<Vec3>& src, const std::vector<Vec3>& dst, const std::vector<Vec3>* nor, double pose16_out[16]) {

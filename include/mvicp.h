@@ -158,6 +158,55 @@ int mvicp_closest_point(mvicp_ctx* ctx, int32_t frame, const double query[3], in
 int mvicp_optimize(mvicp_ctx* ctx, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt,
                    mvicp_lm_summary* summary);
 
+/* ICP_G2O::g2oOptimizer (include/icp-g2o.h:14, icp-g2o.cpp:149-303), the --g2o path of main_multiview.cpp:158-164: one g2o
+ * Edge_V_V_GICP per stored correspondence of every edge with a free end (vertex 0 = dst, vertex 1 = src), VertexSE3 poses,
+ * Levenberg-Marquardt over H + lambda I (no Jacobi scaling), and the reference's outer loop of optimize(iterations_per_call)
+ * calls that stops after more than no_improvement_limit calls without a relative chi2 improvement.  Frame 0 is fixed.  A free
+ * frame without any correspondence is not part of the problem and keeps its pose bit for bit.  DESIGN.md section 2 states
+ * the g2o semantics that are restated here. */
+typedef struct {
+  int32_t iterations_per_call;      /* 100: optimizer.optimize(100), icp-g2o.cpp:271 (the pairwise solvers use 300)  */
+  int32_t max_calls;                /* 100: icp-g2o.cpp:267                                                           */
+  int32_t no_improvement_limit;     /* 5: stop once more than this many calls did not improve chi2, icp-g2o.cpp:297   */
+  int32_t max_trials;               /* 10: g2o's maxTrialsAfterFailure                                                */
+  int32_t orthonormalize_after;     /* 1000: VertexSE3::orthogonalizeAfter                                            */
+  int32_t reserved;
+  double tau;                       /* 1e-5: g2o's initial lambda = tau * max |H_jj|                                  */
+  double information_eps;           /* 0.01: point-to-plane information prec0(eps), icp-g2o.cpp:248                   */
+} mvicp_g2o_options;
+
+enum { MVICP_G2O_END_NO_IMPROVEMENT = 0, /* the outer loop's noImpr counter passed its limit                   */
+       MVICP_G2O_END_MAX_CALLS = 1,      /* max_calls calls of optimize() ran                                   */
+       MVICP_G2O_END_NO_VERTICES = 2     /* no free frame has a correspondence: nothing was optimised           */ };
+enum { MVICP_G2O_CALL_TERMINATE = 0,     /* the last call stopped on g2o's Terminate (trials exhausted or rho == 0) */
+       MVICP_G2O_CALL_ITERATIONS = 1     /* the last call ran all of its iterations                                */ };
+
+typedef struct {
+  int32_t calls;                    /* optimize() calls                                          */
+  int32_t iterations;               /* LM iterations over all calls                              */
+  int32_t trials;                   /* trial steps = linear solves                               */
+  int32_t accepted;                 /* trials kept                                               */
+  int32_t evaluations;              /* streaming passes over the correspondences                 */
+  int32_t ended;                    /* MVICP_G2O_END_*                                           */
+  int32_t last_call_end;            /* MVICP_G2O_CALL_*                                          */
+  int32_t reserved;
+  double chi2_initial, chi2_final;  /* sum e^T Omega e before the first call / after the last    */
+} mvicp_g2o_summary;
+
+void mvicp_default_g2o_options(mvicp_g2o_options* o);
+/* cost: MVICP_COST_P2P or MVICP_COST_P2PLANE (MIXED: MVICP_ERR_INVALID).  Not available in a sharded context (world > 1:
+ * MVICP_ERR_STATE).  chi2_per_call (nullable, >= max_calls + 1 doubles): chi2 before the first call, then after each call. */
+int mvicp_optimize_g2o(mvicp_ctx* ctx, int32_t cost, const mvicp_g2o_options* opt, mvicp_g2o_summary* summary,
+                       double* chi2_per_call);
+/* ICP_G2O::pointToPoint / pointToPlane (include/icp-g2o.h:10-11, icp-g2o.cpp:26-147): dst fixed at the identity, src from the
+ * identity, 1:1 correspondences, one optimize() call of opt->iterations_per_call (opt NULL: 300) iterations, no outer loop.
+ * pose16_out = the src vertex's pose (src -> dst).  nor = dst normals (NULL for point-to-point). */
+int mvicp_pairwise_g2o(const mvicp_config* cfg, int32_t cost, const double* src_xyz, const double* dst_xyz, const double* nor_xyz,
+                       int64_t n, const mvicp_g2o_options* opt, double* pose16_out, mvicp_g2o_summary* summary);
+/* The trial trace of the last mvicp_optimize_g2o: 5 doubles per trial (lambda, chi, tchi, rho, accepted), in order.  Copies
+ * min(capacity, recorded) rows; *n_trials = trials run (the first 65536 are recorded). */
+int mvicp_g2o_trace(mvicp_ctx* ctx, double* out5, int64_t capacity, int64_t* n_trials);
+
 /* One pass of the loop body main_multiview.cpp:150-169 (correspond + optimize). */
 int mvicp_icp_round(mvicp_ctx* ctx, float thresh, int32_t param, int32_t cost, int32_t robust,
                     const mvicp_lm_options* opt, mvicp_lm_summary* summary);

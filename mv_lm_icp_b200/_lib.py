@@ -32,6 +32,21 @@ class LmSummary(C.Structure):
         return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
 
 
+class G2oOptions(C.Structure):
+    _fields_ = [("iterations_per_call", C.c_int32), ("max_calls", C.c_int32), ("no_improvement_limit", C.c_int32),
+                ("max_trials", C.c_int32), ("orthonormalize_after", C.c_int32), ("reserved", C.c_int32),
+                ("tau", C.c_double), ("information_eps", C.c_double)]
+
+
+class G2oSummary(C.Structure):
+    _fields_ = [("calls", C.c_int32), ("iterations", C.c_int32), ("trials", C.c_int32), ("accepted", C.c_int32),
+                ("evaluations", C.c_int32), ("ended", C.c_int32), ("last_call_end", C.c_int32), ("reserved", C.c_int32),
+                ("chi2_initial", C.c_double), ("chi2_final", C.c_double)]
+
+    def asdict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_ if k != "reserved"}
+
+
 class Stats(C.Structure):
     _fields_ = [("knn_ms", C.c_float), ("select_ms", C.c_float), ("lm_eval_ms", C.c_float), ("lm_other_ms", C.c_float),
                 ("correspond_ms", C.c_float), ("optimize_ms", C.c_float),
@@ -47,7 +62,8 @@ EXPORTS = ["mvicp_default_lm_options", "mvicp_last_error", "mvicp_create", "mvic
            "mvicp_set_poses", "mvicp_get_poses", "mvicp_set_graph", "mvicp_pose_graph_knn", "mvicp_get_graph",
            "mvicp_correspond", "mvicp_get_edge", "mvicp_get_all_edges", "mvicp_get_nn", "mvicp_set_edge", "mvicp_closest_point",
            "mvicp_optimize", "mvicp_icp_round", "mvicp_pairwise", "mvicp_pairwise_closed", "mvicp_recompute_normals", "mvicp_get_normals", "mvicp_knn_self", "mvicp_nccl_unique_id", "mvicp_comm_init",
-           "mvicp_get_stats", "mvicp_get_stream", "mvicp_sync", "mvicp_abi_version", "mvicp_host_alloc", "mvicp_host_free"]
+           "mvicp_get_stats", "mvicp_get_stream", "mvicp_sync", "mvicp_abi_version", "mvicp_host_alloc", "mvicp_host_free",
+           "mvicp_default_g2o_options", "mvicp_optimize_g2o", "mvicp_pairwise_g2o", "mvicp_g2o_trace"]
 
 
 def build(force=False):

@@ -1,0 +1,407 @@
+// g2o.cuh -- the reference's g2o backend (src/internal/icp-g2o.cpp) on the device: one Edge_V_V_GICP per correspondence,
+// VertexSE3 poses, OptimizationAlgorithmLevenberg with a dense linear solver, and the multiview outer loop of optimize(100)
+// calls with its no-improvement counter.  Semantics marked [ext] are g2o's (tag 20170730_git), restated in DESIGN section 2.
+//
+// Per correspondence (first, second) of edge src -> dst: vertex 0 = dst (T0 = [F0 | t0]), vertex 1 = src (T1 = [F1 | t1]),
+// pos0 = dst point, pos1 = src point, normal0 = dst normal.
+//   error     e = T0^-1 (T1 pos1) - pos0, T0^-1 = [F0^T | -F0^T t0] (Eigen's isometry inverse, also for non-rigid F0)   [ext]
+//   info      point-to-point: I;  point-to-plane: prec0(eps) = R0^T diag(eps, eps, 1) R0 with R0 from makeRot0(normal0)  [ext]
+//   chi2      sum e^T Omega e (no 1/2, no robust kernel: the reference comments its Huber kernel out, icp-g2o.cpp:152-156)
+//   Jacobians (GICP_ANALYTIC_JACOBIANS, increment order tx ty tz qx qy qz), u = T0^-1 T1 pos1, M01 = F0^T F1            [ext]
+//             J_dst = [ -I | 2 [u]x ],  J_src = [ M01 | -2 M01 [pos1]x ]
+// Streaming kernel: the two-lane split of lm_eval_general_kernel (lm_eval.cuh): lane pairs share a correspondence, the even
+// lane owns the src half of the Jacobian row block, the odd lane the dst half; they accumulate the 12x12 pair matrix directly
+// (correct for non-rigid poses) in lm_eval_general_kernel's partial layout (GBLK).  In a trial evaluation only chi2 is
+// accumulated, with the same lane mapping and reduction order, so a point's chi2 is bit-identical in both modes.
+#pragma once
+#include <cuda_runtime.h>
+#include "../../include/mvicp.h"
+#include "knn.cuh"
+#include "lm_eval.cuh"
+#include "lm_step.cuh"
+#include "se3_math.cuh"
+#include "types.cuh"
+
+namespace mv {
+
+enum { G2O_BUILD = 0, G2O_TRIAL = 1 };   // what the pending evaluation is for
+
+struct G2oState {
+  int32_t M, E, n, max_iter, max_calls, no_impr_limit, max_trials, ortho_after;
+  int32_t phase, done, ended, last_call_end, call, iter, q, no_impr;
+  int32_t n_iters, n_trials, n_accepted, n_evals, n_trace, trace_cap;
+  double tau, lambda, nu, chi, last_chi, chi_initial, scale;
+};
+
+// Omega = R0^T diag(eps, eps, 1) R0 (upper triangle 00 01 02 11 12 22), R0 row by row as EdgeGICP::makeRot0 builds it:
+// row 2 = normal0 (not normalised), row 1 = normalise((0,1,0) - normal0.y normal0), row 0 = normal0 x row 1.
+__host__ __device__ __forceinline__ void g2o_prec0(const double* n, double eps, double* Om) {
+  double y[3] = {-n[1] * n[0], 1.0 - n[1] * n[1], -n[1] * n[2]};
+  const double yy = y[0] * y[0] + y[1] * y[1] + y[2] * y[2];
+  if (yy > 0.0) { const double s = sqrt(yy); y[0] /= s; y[1] /= s; y[2] /= s; }   // Eigen's normalize(): a zero vector stays zero
+  double x[3]; cross(n, y, x);
+  const double* R[3] = {x, y, n};
+  const double d[3] = {eps, eps, 1.0};
+  int k = 0;
+  for (int a = 0; a < 3; ++a)
+    for (int b = a; b < 3; ++b) Om[k++] = (R[0][a] * d[0]) * R[0][b] + (R[1][a] * d[1]) * R[1][b] + (R[2][a] * d[2]) * R[2][b];
+}
+
+template <bool F32, bool NF32, int COST>
+__global__ void __launch_bounds__(EVAL_THREADS)
+g2o_eval_kernel(const FrameDev* __restrict__ frames, const EdgeDev* __restrict__ edges, const Tile* __restrict__ tiles, int tile_len,
+                const int32_t* __restrict__ corr, const Rt* __restrict__ pose_eval, const G2oState* __restrict__ S, double eps,
+                double* __restrict__ partial) {
+  if (S->done) return;   // issued speculatively after the solve terminated
+  const bool build = S->phase == G2O_BUILD;
+  const Tile t = tiles[blockIdx.x];
+  const EdgeDev e = edges[t.edge];
+  __shared__ double sF1[9], st1[3], sF0T[9], smt[3], sM01[9];
+  __shared__ double sred[EVAL_THREADS / 32][2][GACC];
+  if (threadIdx.x == 0) {
+    const Rt a = pose_eval[e.src], k = pose_eval[e.dst];
+    for (int i = 0; i < 9; ++i) sF1[i] = a.R[i];
+    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) sF0T[3 * i + j] = k.R[3 * j + i];
+    double ft[3]; matTvec(k.R, k.t, ft);
+    for (int i = 0; i < 3; ++i) { st1[i] = a.t[i]; smt[i] = -ft[i]; }
+    matTmul(k.R, a.R, sM01);
+  }
+  __syncthreads();
+  const int role = threadIdx.x & 1;   // 0: src half of the row block, 1: dst half
+  // this lane's translation block B and rotation columns s * C (v x e_j):  src (M01, M01, pos1, -2), dst (-I, I, u, 2)
+  double C[9];
+#pragma unroll
+  for (int i = 0; i < 9; ++i) C[i] = role ? ((i % 4 == 0) ? 1.0 : 0.0) : sM01[i];
+  const double tsg = role ? -1.0 : 1.0, rsg = role ? 2.0 : -2.0;
+  const FrameDev fs = frames[e.src];
+  const FrameDev fd = frames[e.dst];
+  double acc[GACC];
+#pragma unroll
+  for (int i = 0; i < GACC; ++i) acc[i] = 0.0;
+  const int end = min(t.start + tile_len, e.n_src);
+  for (int k0 = t.start; k0 < end; k0 += EVAL_THREADS / 2) {   // uniform trip count: the pair shuffles need every lane
+    const int k = k0 + (threadIdx.x >> 1);
+    const int c = k < end ? __ldg(corr + e.off + k) : -1;
+    const bool ok = c >= 0;
+    if (!__any_sync(0xffffffffu, ok)) continue;
+    double p[3] = {0, 0, 0}, q[3] = {0, 0, 0}, n[3] = {0, 0, 0}; int dummy;
+    if (ok) {
+      Rec<F32>::load(fs.pts_o, k, p[0], p[1], p[2], dummy);
+      Rec<F32>::load(fd.pts_o, c, q[0], q[1], q[2], dummy);
+      if (COST == COST_P2PLANE) Rec<NF32>::load(fd.nor_o, c, n[0], n[1], n[2], dummy);
+    }
+    const double live = ok ? 1.0 : 0.0;   // an empty slot adds exact zeros
+    double y[3], u[3], r[3];
+    matvec(sF1, p, y);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) y[i] += st1[i];
+    matvec(sF0T, y, u);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) { u[i] += smt[i]; r[i] = u[i] - q[i]; }
+    double Om[6] = {1, 0, 0, 1, 0, 1};
+    if (COST == COST_P2PLANE) g2o_prec0(n, eps, Om);
+    const double O3[9] = {Om[0], Om[1], Om[2], Om[1], Om[3], Om[4], Om[2], Om[4], Om[5]};
+    double Or[3]; matvec(O3, r, Or);
+    acc[45] += live * (r[0] * Or[0] + r[1] * Or[1] + r[2] * Or[2]);
+    if (!build) continue;
+    // this lane's half J (3 x 6) and W = Omega J
+    const double v[3] = {role ? u[0] : p[0], role ? u[1] : p[1], role ? u[2] : p[2]};
+    const double vx[3][3] = {{0.0, v[2], -v[1]}, {-v[2], 0.0, v[0]}, {v[1], -v[0], 0.0}};   // v x e_j
+    double J[3][6], W[3][6];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        J[i][j] = tsg * C[3 * i + j];
+        J[i][3 + j] = rsg * (C[3 * i] * vx[j][0] + C[3 * i + 1] * vx[j][1] + C[3 * i + 2] * vx[j][2]);
+      }
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+      for (int j = 0; j < 6; ++j) W[i][j] = O3[3 * i] * J[0][j] + O3[3 * i + 1] * J[1][j] + O3[3 * i + 2] * J[2][j];
+    int idx = 0;
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+#pragma unroll
+      for (int b = a; b < 6; ++b) acc[idx++] += live * (J[0][a] * W[0][b] + J[1][a] * W[1][b] + J[2][a] * W[2][b]);
+    // (src, dst) block = J_src^T W_dst: rows 0-2 on the even lane (own J cols 0-2, partner's W), rows 3-5 on the odd lane
+    // (partner's J cols 3-5, own W)
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      double X[3];
+#pragma unroll
+      for (int i = 0; i < 3; ++i) { const double o = __shfl_xor_sync(0xffffffffu, J[i][3 + a], 1); X[i] = role ? o : J[i][a]; }
+#pragma unroll
+      for (int b = 0; b < 6; ++b) {
+        double Y[3];
+#pragma unroll
+        for (int i = 0; i < 3; ++i) { const double o = __shfl_xor_sync(0xffffffffu, W[i][b], 1); Y[i] = role ? W[i][b] : o; }
+        acc[21 + 6 * a + b] += live * (X[0] * Y[0] + X[1] * Y[1] + X[2] * Y[2]);
+      }
+    }
+#pragma unroll
+    for (int a = 0; a < 6; ++a) acc[39 + a] += live * (J[0][a] * Or[0] + J[1][a] * Or[1] + J[2][a] * Or[2]);
+  }
+  // sum over the lanes of equal role (xor 16, 8, 4, 2), then over the warps in order (as lm_eval_general_kernel)
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+#pragma unroll
+  for (int i = 0; i < GACC; ++i) {
+    if (!build && i != 45) continue;
+    double v = acc[i];
+#pragma unroll
+    for (int o = 16; o > 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane < 2) sred[wid][lane][i] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < 2 * GACC) {
+    const int rl = threadIdx.x / GACC, i = threadIdx.x - GACC * rl;
+    if (!build && i != 45) return;
+    double v = 0.0;
+    for (int w = 0; w < EVAL_THREADS / 32; ++w) v += sred[w][rl][i];
+    int dst = -1;
+    if (i < 21) {
+      int a = 0, rem = i; while (rem >= 6 - a) { rem -= 6 - a; ++a; }
+      dst = u12(6 * rl + a, 6 * rl + a + rem);
+    } else if (i < 39) {
+      const int a = (i - 21) / 6, b = (i - 21) - 6 * a;
+      dst = u12(rl ? 3 + a : a, 6 + b);
+    } else if (i < 45) dst = 78 + 6 * rl + (i - 39);
+    else if (rl == 0) dst = 90;
+    if (dst >= 0) partial[(size_t)blockIdx.x * GBLK + dst] = v;
+  }
+}
+
+// One CTA per edge: the edge's tile partials summed in tile order (deterministic) into lm_edge_general_kernel's output layout:
+// pair matrix over [src | dst] (144), pair gradient J^T Omega e (12), chi2 (slot 156).  A trial evaluation sums only chi2.
+__global__ void __launch_bounds__(EDGE_THREADS)
+g2o_edge_kernel(const int32_t* __restrict__ edge_tile_begin, const double* __restrict__ partial, const G2oState* __restrict__ S,
+                double* __restrict__ out) {
+  if (S->done) return;
+  const bool build = S->phase == G2O_BUILD;
+  const int e = blockIdx.x, tid = threadIdx.x;
+  __shared__ double blk[GBLK];
+  double* o = out + (size_t)EOUT_ * e;
+  for (int j = tid; j < 91; j += EDGE_THREADS) {
+    if (!build && j != 90) continue;
+    double v = 0.0;
+    for (int t = edge_tile_begin[e]; t < edge_tile_begin[e + 1]; ++t) v += partial[(size_t)t * GBLK + j];
+    blk[j] = v;
+  }
+  __syncthreads();
+  if (!build) { if (tid == 0) o[156] = blk[90]; return; }
+  for (int r = tid; r < 157; r += EDGE_THREADS) {
+    if (r < 144) { const int a = r / 12, b = r - 12 * a; o[r] = blk[u12(min(a, b), max(a, b))]; }
+    else if (r < 156) o[r] = blk[78 + (r - 144)];
+    else o[r] = blk[90];
+  }
+}
+
+// inliers per edge (corr >= 0) over the g2o tile list: which vertices take part in the problem
+__global__ void g2o_count_kernel(const EdgeDev* __restrict__ edges, const Tile* __restrict__ tiles, int tile_len, const int32_t* __restrict__ corr,
+                                 unsigned long long* __restrict__ count) {
+  const Tile t = tiles[blockIdx.x];
+  const EdgeDev e = edges[t.edge];
+  const int end = min(t.start + tile_len, e.n_src);
+  int m = 0;
+  for (int k = t.start + threadIdx.x; k < end; k += blockDim.x) m += __ldg(corr + e.off + k) >= 0 ? 1 : 0;
+  if (m) atomicAdd(count + t.edge, (unsigned long long)m);
+}
+
+struct G2oWork {
+  G2oState* S;
+  const double* eout;            // [E][EOUT] from g2o_edge_kernel
+  volatile int32_t* host_flag;   // mapped pinned ring: (sequence << 1) | done
+  int32_t seq;
+  Rt* x;                         // [M] current estimate of every vertex
+  Rt* ev;                        // [M] evaluation point: x (build) or the trial estimate
+  int32_t* n_oplus;              // [M] VertexSE3::_numOplusCalls
+  const int32_t* col;            // [M] first column or -1 (fixed, or no correspondence)
+  const int32_t* hb_ptr; const int32_t* hb_row; const int32_t* hb_col; const int32_t* hc_edge; const int32_t* hc_sub; int32_t n_hblocks;
+  const int32_t* gb_ptr; const int32_t* gc_edge; const int32_t* gc_side;
+  const int32_t* rlast; const int32_t* rfirst; const int32_t* rowbase;
+  double *H, *b, *Lg, *rhs;
+  double* poses16;
+  double* chi_calls;             // [max_calls + 1]: chi2 before the first call, then after every call
+  double* trace;                 // [trace_cap][5]: lambda, chi, tchi, rho, accepted -- one row per trial
+  int32_t l_in_smem;
+};
+
+__global__ void g2o_init_kernel(G2oWork w, int M) {
+  const int f = blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= M) return;
+  Rt a; pose16_to_Rt(w.poses16 + 16 * f, &a);
+  w.x[f] = a; w.ev[f] = a; w.n_oplus[f] = 0;
+}
+
+// VertexSE3::oplusImpl [ext]: T <- T [R(q) | t] with (t, qx, qy, qz) = d, qw = sqrt(1 - |q|^2) (identity rotation if |q|^2 > 1),
+// Eigen's Quaternion::toRotationMatrix; after more than `ortho_after` updates F <- F - F (F^T F - I) / 2 and the count restarts.
+__device__ __forceinline__ void g2o_oplus(const Rt& x, const double* d, int* count, int ortho_after, Rt* out) {
+  const double qq = d[3] * d[3] + d[4] * d[4] + d[5] * d[5];
+  double R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+  if (!(1.0 - qq < 0.0)) {
+    const double qw = sqrt(1.0 - qq), qx = d[3], qy = d[4], qz = d[5];
+    const double tx = 2 * qx, ty = 2 * qy, tz = 2 * qz;
+    const double twx = tx * qw, twy = ty * qw, twz = tz * qw, txx = tx * qx, txy = ty * qx, txz = tz * qx, tyy = ty * qy, tyz = tz * qy, tzz = tz * qz;
+    R[0] = 1 - (tyy + tzz); R[1] = txy - twz; R[2] = txz + twy;
+    R[3] = txy + twz; R[4] = 1 - (txx + tzz); R[5] = tyz - twx;
+    R[6] = txz - twy; R[7] = tyz + twx; R[8] = 1 - (txx + tyy);
+  }
+  matmul(x.R, R, out->R);
+  matvec(x.R, d, out->t);
+  for (int i = 0; i < 3; ++i) out->t[i] += x.t[i];
+  if (++*count > ortho_after) {
+    *count = 0;
+    double Em[9]; matTmul(out->R, out->R, Em);
+    Em[0] -= 1; Em[4] -= 1; Em[8] -= 1;
+    double FE[9]; matmul(out->R, Em, FE);
+    for (int i = 0; i < 9; ++i) out->R[i] -= 0.5 * FE[i];
+  }
+}
+
+// OptimizationAlgorithmLevenberg::solve + SparseOptimizer::optimize + the reference's outer loop (icp-g2o.cpp:261-303), one CTA.
+// Every launch consumes one evaluation (S->phase says which kind), runs trials that need no evaluation (a failed factorisation),
+// and leaves the next evaluation point in ev.
+__global__ void __launch_bounds__(STEP_THREADS) g2o_step_kernel(G2oWork w) {
+  extern __shared__ double smem[];
+  __shared__ double red[40];
+  __shared__ G2oState s_state;
+  __shared__ int s_solve, s_accept, s_tobuild;
+  if (w.S->done) { if (threadIdx.x == 0) { w.host_flag[w.seq & 7] = (w.seq << 1) | 1; __threadfence_system(); } return; }
+  const int tid = threadIdx.x, T = blockDim.x;
+  for (int i = tid; i < (int)(sizeof(G2oState) / sizeof(int32_t)); i += T)
+    reinterpret_cast<int32_t*>(&s_state)[i] = reinterpret_cast<const int32_t*>(w.S)[i];
+  __syncthreads();
+  G2oState* S = &s_state;
+  const int n = S->n, M = S->M, E = S->E;
+  const int phase = S->phase;   // thread 0 moves S->phase on below
+  double* colj = smem; double* dg = smem + 2 * (n + 1);
+  double* L = w.l_in_smem ? smem + 3 * (n + 1) : w.Lg;
+
+  double chi_eval = 0.0;   // edges summed in a fixed order
+  for (int e = tid; e < E; e += T) chi_eval += w.eout[(size_t)EOUT * e + 156];
+  chi_eval = block_sum(chi_eval, red);
+
+  // end of an iteration (Terminate: trials exhausted or rho == 0), of a call (SparseOptimizer::optimize), of the outer loop
+  auto end_iter = [&](double rho) {   // thread 0 only
+    S->iter += 1; S->n_iters += 1;
+    const bool term = S->q == S->max_trials || rho == 0.0;
+    if (term || S->iter >= S->max_iter) {
+      S->last_call_end = term ? MVICP_G2O_CALL_TERMINATE : MVICP_G2O_CALL_ITERATIONS;
+      w.chi_calls[S->call + 1] = S->chi;   // computeActiveErrors(); chi2() at the call's final estimate
+      const double impr = (S->last_chi - S->chi) / S->last_chi;
+      S->last_chi = S->chi;
+      if (!(impr > 0.0)) S->no_impr += 1;
+      S->call += 1;
+      if (S->no_impr > S->no_impr_limit) { S->done = 1; S->ended = MVICP_G2O_END_NO_IMPROVEMENT; return; }
+      if (S->call >= S->max_calls) { S->done = 1; S->ended = MVICP_G2O_END_MAX_CALLS; return; }
+      S->iter = 0;
+    }
+    S->phase = G2O_BUILD;
+    s_tobuild = 1;
+  };
+  auto record = [&](double tchi, double rho, bool acc) {   // thread 0 only
+    if (S->n_trace < S->trace_cap) {
+      double* r = w.trace + 5 * (size_t)S->n_trace;
+      r[0] = S->lambda; r[1] = S->chi; r[2] = tchi; r[3] = rho; r[4] = acc ? 1.0 : 0.0;
+    }
+    S->n_trace += 1;
+  };
+
+  if (tid == 0) { s_solve = 0; s_accept = 0; s_tobuild = 0; S->n_evals += 1; }
+  if (phase == G2O_BUILD) {
+    // H = sum J^T Omega J over the listed blocks, b = -sum J^T Omega e
+    for (int idx = tid; idx < w.n_hblocks * 36; idx += T) {
+      const int bk = idx / 36, r = idx - 36 * bk, i = r / 6, j = r - 6 * i;
+      double s = 0;
+      for (int c = w.hb_ptr[bk]; c < w.hb_ptr[bk + 1]; ++c) {
+        const int e = w.hc_edge[c], sub = w.hc_sub[c];   // sub: 0 ss, 1 sk, 2 ks, 3 kk
+        s += w.eout[(size_t)EOUT * e + (6 * (sub >> 1) + i) * 12 + 6 * (sub & 1) + j];
+      }
+      w.H[(size_t)(w.hb_row[bk] + i) * n + w.hb_col[bk] + j] = s;
+    }
+    for (int idx = tid; idx < M * 6; idx += T) {
+      const int f = idx / 6, i = idx - 6 * f;
+      if (w.col[f] < 0) continue;
+      double s = 0;
+      for (int c = w.gb_ptr[f]; c < w.gb_ptr[f + 1]; ++c) s += w.eout[(size_t)EOUT * w.gc_edge[c] + 144 + 6 * w.gc_side[c] + i];
+      w.b[w.col[f] + i] = -s;
+    }
+    __syncthreads();
+    double md = 0.0;
+    for (int j = tid; j < n; j += T) md = fmax(md, fabs(w.H[(size_t)j * n + j]));
+    md = block_max(md, red);
+    if (tid == 0) {
+      if (S->call == 0 && S->iter == 0) { S->chi_initial = S->last_chi = chi_eval; w.chi_calls[0] = chi_eval; }
+      S->chi = chi_eval;
+      if (S->iter == 0) { S->lambda = S->tau * md; S->nu = 2.0; }   // computeLambdaInit at iteration 0 of every call
+      S->q = 0;
+      s_solve = 1;
+    }
+  } else if (tid == 0) {   // a trial's chi2
+    const double tchi = chi_eval;
+    const double rho = (S->chi - tchi) / S->scale;
+    const bool acc = rho > 0.0 && isfinite(tchi);
+    record(tchi, rho, acc);
+    if (acc) {
+      const double a = 1.0 - (2.0 * rho - 1.0) * (2.0 * rho - 1.0) * (2.0 * rho - 1.0);
+      S->lambda *= fmax(1.0 / 3.0, fmin(2.0 / 3.0, a));
+      S->nu = 2.0; S->chi = tchi; S->n_accepted += 1;
+      s_accept = 1;
+    } else { S->lambda *= S->nu; S->nu *= 2.0; }
+    S->q += 1;
+    if (rho < 0.0 && S->q < S->max_trials) s_solve = 1; else end_iter(rho);
+  }
+  __syncthreads();
+  if (s_accept) for (int f = tid; f < M; f += T) w.x[f] = w.ev[f];   // keep the trial (discardTop); otherwise pop
+  __syncthreads();
+
+  while (s_solve) {
+    // (H + lambda I) dx = b, skyline Cholesky of lm_step.cuh
+    const double lambda = S->lambda;
+    for (int i = tid >> 5; i < n; i += T >> 5) {
+      const int rbi = w.rowbase[i];
+      for (int j = w.rfirst[i] + (tid & 31); j <= i; j += 32) L[rbi + j] = w.H[(size_t)i * n + j] + (i == j ? lambda : 0.0);
+    }
+    { const int rbn = w.rowbase[n]; for (int j = tid; j < n; j += T) L[rbn + j] = w.b[j]; }
+    __syncthreads();
+    bool ok = chol_solve(L, w.rowbase, n, colj, dg, w.rhs, w.rlast, w.rfirst);
+    double bad = 0.0;
+    if (ok) for (int j = tid; j < n; j += T) if (!isfinite(w.rhs[j])) bad = 1.0;
+    bad = block_sum(bad, red);
+    ok = ok && bad == 0.0;
+    double sc = 0.0;
+    if (ok) for (int j = tid; j < n; j += T) sc += w.rhs[j] * (lambda * w.rhs[j] + w.b[j]);
+    sc = block_sum(sc, red);   // computeScale()
+    // the update is applied to every vertex in the problem (and counted) even when the factorisation failed; it is undone then
+    for (int f = tid; f < M; f += T) {
+      const int cf = w.col[f];
+      if (cf < 0) continue;
+      Rt nx;
+      g2o_oplus(w.x[f], w.rhs + cf, &w.n_oplus[f], S->ortho_after, &nx);
+      if (ok) w.ev[f] = nx;
+    }
+    __syncthreads();
+    if (tid == 0) {
+      S->n_trials += 1;
+      s_solve = 0;
+      if (ok) { S->scale = sc + 1e-3; S->phase = G2O_TRIAL; }
+      else {   // a non-positive pivot: tchi = +inf, a rejected trial without an evaluation
+        const double rho = -INFINITY;
+        record(INFINITY, rho, false);
+        S->lambda *= S->nu; S->nu *= 2.0; S->q += 1;
+        if (S->q < S->max_trials) s_solve = 1; else end_iter(rho);
+      }
+    }
+    __syncthreads();
+  }
+  if (s_tobuild && !S->done) for (int f = tid; f < M; f += T) w.ev[f] = w.x[f];
+  if (S->done)   // write the vertices of the problem back; every other frame keeps its pose bit for bit
+    for (int f = tid; f < M; f += T) if (w.col[f] >= 0) Rt_to_pose16(&w.x[f], w.poses16 + 16 * f);
+  __syncthreads();
+  for (int i = tid; i < (int)(sizeof(G2oState) / sizeof(int32_t)); i += T)
+    reinterpret_cast<int32_t*>(w.S)[i] = reinterpret_cast<const int32_t*>(&s_state)[i];
+  __syncthreads();
+  if (tid == 0) { __threadfence(); w.host_flag[w.seq & 7] = (w.seq << 1) | (S->done ? 1 : 0); __threadfence_system(); }
+}
+
+}  // namespace mv

@@ -25,6 +25,7 @@
 #include "closed.cuh"
 #include "compact.cuh"
 #include "far.cuh"
+#include "g2o.cuh"
 #include "knn.cuh"
 #include "lm_eval.cuh"
 #include "lm_step.cuh"
@@ -120,6 +121,9 @@ struct mvicp_ctx {
   void* h_state = nullptr;     // pinned staging of LmState
   volatile int32_t* h_flag = nullptr; volatile int32_t* d_flag = nullptr;   // mapped pinned ring written by lm_step_kernel
   std::vector<uint8_t> lm_key; uint32_t graph_gen = 0;
+  // g2o solve (g2o.cuh); shares the normal-matrix buffers above and clears lm_key when it has used them
+  DevBuf d_g2o_state, d_g2o_x, d_g2o_ev, d_g2o_nop, d_g2o_chi, d_g2o_trace, d_g2o_tiles, d_g2o_tile_begin, d_g2o_cnt;
+  int64_t g2o_trials = 0;
   // stats
   mvicp_stats stats{};
   cudaEvent_t ev[8]{};
@@ -381,7 +385,9 @@ void mvicp_destroy(mvicp_ctx* c) {
                     &c->d_state, &c->d_x, &c->d_cand, &c->d_Rt, &c->d_K, &c->d_col, &c->d_H, &c->d_g, &c->d_Hc,
                     &c->d_gc, &c->d_scale, &c->d_diag, &c->d_L, &c->d_rhs, &c->d_step, &c->d_eout,
                     &c->d_hb_ptr, &c->d_hb_row, &c->d_hb_col, &c->d_hc_edge, &c->d_hc_sub, &c->d_gb_ptr, &c->d_gc_edge,
-                    &c->d_gc_side, &c->d_posegather, &c->d_rlast, &c->d_rfirst, &c->d_rowbase, &c->d_gen, &c->d_obb, &c->d_single, &c->d_prof, &c->d_tile_count, &c->d_tile_off, &c->d_edge_off, &c->d_recs};
+                    &c->d_gc_side, &c->d_posegather, &c->d_rlast, &c->d_rfirst, &c->d_rowbase, &c->d_gen, &c->d_obb, &c->d_single, &c->d_prof, &c->d_tile_count, &c->d_tile_off, &c->d_edge_off, &c->d_recs,
+                    &c->d_g2o_state, &c->d_g2o_x, &c->d_g2o_ev, &c->d_g2o_nop, &c->d_g2o_chi, &c->d_g2o_trace, &c->d_g2o_tiles,
+                    &c->d_g2o_tile_begin, &c->d_g2o_cnt};
   for (DevBuf* b : bufs) b->release();
   for (auto& ev : c->ev) if (ev) cudaEventDestroy(ev);
   for (auto& ev : c->eval_ev) cudaEventDestroy(ev);
@@ -899,6 +905,56 @@ static int prepare_lm(mvicp_ctx* c, int n) {
   return MVICP_OK;
 }
 
+// Block structure of the normal matrix over n local columns (c->h_col): blk[r * M + q] lists the (edge, sub-block) pairs that
+// sum into block (r, q) (sub 0 ss, 1 sk, 2 ks, 3 kk of the edge's pair matrix), gl[f] the (edge, side) pairs of frame f's
+// gradient.  Uploads the gather lists, the envelope and the skyline layout of the factor, and zeroes the dense matrices.
+typedef std::vector<std::vector<std::pair<int, int>>> BlockLists;
+static int upload_lm_structure(mvicp_ctx* c, int n, const BlockLists& blk, const BlockLists& gl) {
+  const int M = c->M;
+  std::vector<int32_t> hb_ptr{0}, hb_row, hb_col, hc_edge, hc_sub, gb_ptr{0}, gc_edge, gc_side;
+  for (int r = 0; r < M; ++r)
+    for (int q = 0; q < M; ++q) {
+      const auto& l = blk[(size_t)r * M + q];
+      if (l.empty()) continue;
+      hb_row.push_back(c->h_col[r]); hb_col.push_back(c->h_col[q]);
+      for (auto& pr : l) { hc_edge.push_back(pr.first); hc_sub.push_back(pr.second); }
+      hb_ptr.push_back((int32_t)hc_edge.size());
+    }
+  for (int f = 0; f < M; ++f) { for (auto& pr : gl[f]) { gc_edge.push_back(pr.first); gc_side.push_back(pr.second); } gb_ptr.push_back((int32_t)gc_edge.size()); }
+  c->n_hblocks = (int)hb_row.size();
+  // envelope: first structurally non-zero column of every row, and the last row that reaches column j
+  std::vector<int32_t> rfirst(n), rlast(n);
+  for (int r = 0; r < n; ++r) rfirst[r] = (r / 6) * 6;
+  for (int b = 0; b < c->n_hblocks; ++b)
+    if (hb_col[b] < hb_row[b]) for (int i = 0; i < 6; ++i) rfirst[hb_row[b] + i] = std::min(rfirst[hb_row[b] + i], hb_col[b]);
+  for (int j = 0; j < n; ++j) { rlast[j] = j; }
+  for (int r = 0; r < n; ++r) for (int j = rfirst[r]; j <= r; ++j) rlast[j] = std::max(rlast[j], r);
+  for (int j = 1; j < n; ++j) rlast[j] = std::max(rlast[j], rlast[j - 1]);   // monotone (fill-in stays inside)
+  auto up = [&](DevBuf& b, const std::vector<int32_t>& v) -> int {
+    RET(b.reserve(sizeof(int32_t) * std::max<size_t>(1, v.size())));
+    if (!v.empty()) CU(cudaMemcpyAsync(b.p, v.data(), sizeof(int32_t) * v.size(), cudaMemcpyHostToDevice, c->stream));
+    return MVICP_OK;
+  };
+  RET(up(c->d_hb_ptr, hb_ptr)); RET(up(c->d_hb_row, hb_row)); RET(up(c->d_hb_col, hb_col)); RET(up(c->d_hc_edge, hc_edge));
+  RET(up(c->d_hc_sub, hc_sub)); RET(up(c->d_gb_ptr, gb_ptr)); RET(up(c->d_gc_edge, gc_edge)); RET(up(c->d_gc_side, gc_side));
+  RET(up(c->d_col, c->h_col));
+  RET(up(c->d_rlast, rlast)); RET(up(c->d_rfirst, rfirst));
+  // skyline storage of the Cholesky factor: row r keeps columns rfirst[r]..r, the rhs row all n
+  std::vector<int32_t> rowbase(n + 1); int64_t at = 0;
+  for (int r = 0; r < n; ++r) { rowbase[r] = (int32_t)(at - rfirst[r]); at += r - rfirst[r] + 1; }
+  rowbase[n] = (int32_t)at; at += n;
+  if (at > INT32_MAX) return fail(MVICP_ERR_INVALID, "normal matrix too large");
+  c->l_size = at;
+  RET(c->d_L.reserve(sizeof(double) * (size_t)at));
+  RET(up(c->d_rowbase, rowbase));
+  // the step kernel writes only the listed blocks of the dense normal matrix; everything else stays zero from here
+  CU(cudaMemsetAsync(c->d_H.p, 0, sizeof(double) * (size_t)n * n, c->stream));
+  CU(cudaMemsetAsync(c->d_Hc.p, 0, sizeof(double) * (size_t)n * n, c->stream));
+
+  CU(cudaStreamSynchronize(c->stream));   // the host vectors above must outlive their copies
+  return MVICP_OK;
+}
+
 }  // extern "C"
 template <bool F32> static void launch_eval(mvicp_ctx* c, int cost, int robust, const int* done_flag) {
   const int nt = c->n_eval_tiles;
@@ -969,47 +1025,7 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
         gl[k].push_back({e, 1});
       }
     }
-    std::vector<int32_t> hb_ptr{0}, hb_row, hb_col, hc_edge, hc_sub, gb_ptr{0}, gc_edge, gc_side;
-    for (int r = 0; r < M; ++r)
-      for (int q = 0; q < M; ++q) {
-        const auto& l = blk[(size_t)r * M + q];
-        if (l.empty()) continue;
-        hb_row.push_back(c->h_col[r]); hb_col.push_back(c->h_col[q]);
-        for (auto& pr : l) { hc_edge.push_back(pr.first); hc_sub.push_back(pr.second); }
-        hb_ptr.push_back((int32_t)hc_edge.size());
-      }
-    for (int f = 0; f < M; ++f) { for (auto& pr : gl[f]) { gc_edge.push_back(pr.first); gc_side.push_back(pr.second); } gb_ptr.push_back((int32_t)gc_edge.size()); }
-    c->n_hblocks = (int)hb_row.size();
-    // envelope: first structurally non-zero column of every row, and the last row that reaches column j
-    std::vector<int32_t> rfirst(n), rlast(n);
-    for (int r = 0; r < n; ++r) rfirst[r] = (r / 6) * 6;
-    for (int b = 0; b < c->n_hblocks; ++b)
-      if (hb_col[b] < hb_row[b]) for (int i = 0; i < 6; ++i) rfirst[hb_row[b] + i] = std::min(rfirst[hb_row[b] + i], hb_col[b]);
-    for (int j = 0; j < n; ++j) { rlast[j] = j; }
-    for (int r = 0; r < n; ++r) for (int j = rfirst[r]; j <= r; ++j) rlast[j] = std::max(rlast[j], r);
-    for (int j = 1; j < n; ++j) rlast[j] = std::max(rlast[j], rlast[j - 1]);   // monotone (fill-in stays inside)
-    auto up = [&](DevBuf& b, const std::vector<int32_t>& v) -> int {
-      RET(b.reserve(sizeof(int32_t) * std::max<size_t>(1, v.size())));
-      if (!v.empty()) CU(cudaMemcpyAsync(b.p, v.data(), sizeof(int32_t) * v.size(), cudaMemcpyHostToDevice, c->stream));
-      return MVICP_OK;
-    };
-    RET(up(c->d_hb_ptr, hb_ptr)); RET(up(c->d_hb_row, hb_row)); RET(up(c->d_hb_col, hb_col)); RET(up(c->d_hc_edge, hc_edge));
-    RET(up(c->d_hc_sub, hc_sub)); RET(up(c->d_gb_ptr, gb_ptr)); RET(up(c->d_gc_edge, gc_edge)); RET(up(c->d_gc_side, gc_side));
-    RET(up(c->d_col, c->h_col));
-    RET(up(c->d_rlast, rlast)); RET(up(c->d_rfirst, rfirst));
-    // skyline storage of the Cholesky factor: row r keeps columns rfirst[r]..r, the rhs row all n
-    std::vector<int32_t> rowbase(n + 1); int64_t at = 0;
-    for (int r = 0; r < n; ++r) { rowbase[r] = (int32_t)(at - rfirst[r]); at += r - rfirst[r] + 1; }
-    rowbase[n] = (int32_t)at; at += n;
-    if (at > INT32_MAX) return fail(MVICP_ERR_INVALID, "normal matrix too large");
-    c->l_size = at;
-    RET(c->d_L.reserve(sizeof(double) * (size_t)at));
-    RET(up(c->d_rowbase, rowbase));
-    // the step kernel writes only the listed blocks of the dense normal matrix; everything else stays zero from here
-    CU(cudaMemsetAsync(c->d_H.p, 0, sizeof(double) * (size_t)n * n, c->stream));
-    CU(cudaMemsetAsync(c->d_Hc.p, 0, sizeof(double) * (size_t)n * n, c->stream));
-
-    CU(cudaStreamSynchronize(c->stream));   // the host vectors above must outlive their copies
+    RET(upload_lm_structure(c, n, blk, gl));
     c->lm_key = key;
   }
   LmState st; std::memset(&st, 0, sizeof st);
@@ -1178,6 +1194,212 @@ int mvicp_pairwise(const mvicp_config* cfg, int32_t param, int32_t cost, const d
   mvicp_destroy(c);
   g_err = keep;
   return rc;
+}
+
+}  // extern "C"
+// ---- g2o backend (g2o.cuh; icp-g2o.cpp) ---------------------------------------------------------------------
+template <bool F32> static void launch_g2o_eval(mvicp_ctx* c, int cost, int nt, const G2oState* S, double eps) {
+#define MV_G2O(NF, COSTK)                                                                                          \
+  g2o_eval_kernel<F32, NF, COSTK><<<nt, EVAL_THREADS, 0, c->stream>>>(c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), \
+      c->d_g2o_tiles.as<Tile>(), c->eval_tile_len, c->d_corr.as<int32_t>(), c->d_g2o_ev.as<Rt>(), S, eps, c->d_partial.as<double>())
+  if (cost == COST_P2P) MV_G2O(F32, COST_P2P);
+  else if (F32 && c->nor_f32) MV_G2O(F32, COST_P2PLANE);
+  else MV_G2O(false, COST_P2PLANE);
+#undef MV_G2O
+}
+static constexpr int G2O_TRACE_CAP = 65536;   // trials whose (lambda, chi, tchi, rho, accepted) row mvicp_g2o_trace returns
+
+extern "C" {
+void mvicp_default_g2o_options(mvicp_g2o_options* o) {
+  o->iterations_per_call = 100; o->max_calls = 100; o->no_improvement_limit = 5; o->max_trials = 10; o->orthonormalize_after = 1000;
+  o->reserved = 0; o->tau = 1e-5; o->information_eps = 0.01;
+}
+
+int mvicp_optimize_g2o(mvicp_ctx* c, int32_t cost, const mvicp_g2o_options* opt_in, mvicp_g2o_summary* summary, double* chi2_per_call) {
+  if (!c || !c->M || !c->E) return fail(MVICP_ERR_STATE, "mvicp_optimize_g2o: frames and graph must be set first");
+  if (cost != COST_P2P && cost != COST_P2PLANE) return fail(MVICP_ERR_INVALID, "mvicp_optimize_g2o: cost must be point-to-point or point-to-plane");
+  if (cost == COST_P2PLANE && !c->have_normals) return fail(MVICP_ERR_INVALID, "point-to-plane needs normals for every frame");
+  if (c->world > 1) return fail(MVICP_ERR_STATE, "mvicp_optimize_g2o: the g2o solve runs on one GPU; this context is sharded");
+  mvicp_g2o_options opt; if (opt_in) opt = *opt_in; else mvicp_default_g2o_options(&opt);
+  if (opt.iterations_per_call < 1 || opt.max_calls < 1 || opt.max_trials < 1 || opt.no_improvement_limit < 0 || opt.orthonormalize_after < 0)
+    return fail(MVICP_ERR_INVALID, "mvicp_optimize_g2o: bad options");
+  CU(cudaSetDevice(c->device));
+  const int M = c->M, E = c->E;
+  c->fixed[0] = 1;   // frames[0]->fixed = true (icp-g2o.cpp:182-186)
+  bool stale = false;
+  for (int e = 0; e < E; ++e) if ((c->edge_owner[e] < 0) != (c->fixed[c->h_edges[e].src] != 0)) stale = true;
+  if (stale) RET(refresh_after_fixed_change(c));
+  // every edge with a free end carries one GICP edge per stored correspondence (an edge between fixed vertices is not active)
+  const int tl = c->eval_tile_len;
+  std::vector<Tile> tiles; std::vector<int32_t> tb(E + 1, 0);
+  for (int e = 0; e < E; ++e) {
+    tb[e] = (int32_t)tiles.size();
+    const EdgeDev& ed = c->h_edges[e];
+    if (c->fixed[ed.src] && c->fixed[ed.dst]) continue;
+    for (int s = 0; s < ed.n_src; s += tl) tiles.push_back(Tile{e, s});
+  }
+  tb[E] = (int32_t)tiles.size();
+  const int nt = (int)tiles.size();
+  RET(c->d_g2o_tiles.reserve(sizeof(Tile) * std::max(1, nt)));
+  RET(c->d_g2o_tile_begin.reserve(sizeof(int32_t) * (E + 1)));
+  RET(c->d_g2o_cnt.reserve(sizeof(unsigned long long) * E));
+  RET(c->d_partial.reserve(sizeof(double) * GBLK * std::max(1, nt)));
+  if (nt) CU(cudaMemcpyAsync(c->d_g2o_tiles.p, tiles.data(), sizeof(Tile) * nt, cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemcpyAsync(c->d_g2o_tile_begin.p, tb.data(), sizeof(int32_t) * (E + 1), cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemsetAsync(c->d_g2o_cnt.p, 0, sizeof(unsigned long long) * E, c->stream));
+  if (nt) {
+    g2o_count_kernel<<<nt, 256, 0, c->stream>>>(c->d_edges.as<EdgeDev>(), c->d_g2o_tiles.as<Tile>(), tl, c->d_corr.as<int32_t>(),
+                                                c->d_g2o_cnt.as<unsigned long long>());
+    c->stats.kernel_launches += 1;
+  }
+  std::vector<unsigned long long> cnt(E);
+  CU(cudaMemcpyAsync(cnt.data(), c->d_g2o_cnt.p, sizeof(unsigned long long) * E, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  // the problem's vertices: free frames with at least one correspondence (a vertex without edges is not optimised)
+  std::vector<uint8_t> touched(M, 0);
+  for (int e = 0; e < E; ++e) if (cnt[e]) { touched[c->h_edges[e].src] = 1; touched[c->h_edges[e].dst] = 1; }
+  c->h_col.assign(M, -1); int n = 0;
+  for (int f = 0; f < M; ++f) if (touched[f] && !c->fixed[f]) { c->h_col[f] = n; n += 6; }
+  if (summary) std::memset(summary, 0, sizeof *summary);
+  c->g2o_trials = 0;
+  if (n == 0) {   // no active edge: chi2 = 0 (g2o's optimize() returns at once, "0 vertices to optimize"), nothing moves
+    if (summary) summary->ended = MVICP_G2O_END_NO_VERTICES;
+    if (chi2_per_call) chi2_per_call[0] = 0.0;
+    return MVICP_OK;
+  }
+  BlockLists blk((size_t)M * M), gl(M);
+  for (int e = 0; e < E; ++e) {
+    if (!cnt[e]) continue;
+    const int s = c->h_edges[e].src, k = c->h_edges[e].dst;
+    const bool fs = c->h_col[s] >= 0, fk = c->h_col[k] >= 0;
+    if (fs) { blk[(size_t)s * M + s].push_back({e, 0}); gl[s].push_back({e, 0}); }
+    if (fs && fk) { blk[(size_t)s * M + k].push_back({e, 1}); blk[(size_t)k * M + s].push_back({e, 2}); }
+    if (fk) { blk[(size_t)k * M + k].push_back({e, 3}); gl[k].push_back({e, 1}); }
+  }
+  RET(prepare_lm(c, n));
+  RET(upload_lm_structure(c, n, blk, gl));
+  c->lm_key.clear();   // the buffers now hold the g2o structure: the next mvicp_optimize rebuilds its own
+  RET(c->d_g2o_state.reserve(sizeof(G2oState)));
+  RET(c->d_g2o_x.reserve(sizeof(Rt) * M)); RET(c->d_g2o_ev.reserve(sizeof(Rt) * M)); RET(c->d_g2o_nop.reserve(sizeof(int32_t) * M));
+  RET(c->d_g2o_chi.reserve(sizeof(double) * (opt.max_calls + 1)));
+  RET(c->d_g2o_trace.reserve(sizeof(double) * 5 * G2O_TRACE_CAP));
+  G2oState st; std::memset(&st, 0, sizeof st);
+  st.M = M; st.E = E; st.n = n; st.max_iter = opt.iterations_per_call; st.max_calls = opt.max_calls;
+  st.no_impr_limit = opt.no_improvement_limit; st.max_trials = opt.max_trials; st.ortho_after = opt.orthonormalize_after;
+  st.phase = G2O_BUILD; st.trace_cap = G2O_TRACE_CAP; st.tau = opt.tau;
+  CU(cudaMemcpyAsync(c->d_g2o_state.p, &st, sizeof st, cudaMemcpyHostToDevice, c->stream));
+  G2oState* dS = c->d_g2o_state.as<G2oState>();
+
+  G2oWork w{};
+  w.S = dS; w.eout = c->d_eout.as<double>(); w.host_flag = c->d_flag;
+  w.x = c->d_g2o_x.as<Rt>(); w.ev = c->d_g2o_ev.as<Rt>(); w.n_oplus = c->d_g2o_nop.as<int32_t>(); w.col = c->d_col.as<int32_t>();
+  w.hb_ptr = c->d_hb_ptr.as<int32_t>(); w.hb_row = c->d_hb_row.as<int32_t>(); w.hb_col = c->d_hb_col.as<int32_t>();
+  w.hc_edge = c->d_hc_edge.as<int32_t>(); w.hc_sub = c->d_hc_sub.as<int32_t>(); w.n_hblocks = c->n_hblocks;
+  w.gb_ptr = c->d_gb_ptr.as<int32_t>(); w.gc_edge = c->d_gc_edge.as<int32_t>(); w.gc_side = c->d_gc_side.as<int32_t>();
+  w.rlast = c->d_rlast.as<int32_t>(); w.rfirst = c->d_rfirst.as<int32_t>(); w.rowbase = c->d_rowbase.as<int32_t>();
+  w.H = c->d_H.as<double>(); w.b = c->d_g.as<double>(); w.Lg = c->d_L.as<double>(); w.rhs = c->d_rhs.as<double>();
+  w.poses16 = c->d_poses.as<double>(); w.chi_calls = c->d_g2o_chi.as<double>(); w.trace = c->d_g2o_trace.as<double>();
+  const size_t l_bytes = sizeof(double) * (size_t)c->l_size;
+  const size_t vec_bytes = sizeof(double) * 3 * (size_t)(n + 1);
+  w.l_in_smem = (l_bytes + vec_bytes) <= 220 * 1024 ? 1 : 0;
+  const size_t dyn = vec_bytes + (w.l_in_smem ? l_bytes : 0);
+  CU(cudaFuncSetAttribute(g2o_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+
+  CU(cudaEventRecord(c->ev[3], c->stream));
+  g2o_init_kernel<<<(M + 63) / 64, 64, 0, c->stream>>>(w, M);
+  c->stats.kernel_launches += 1;
+  // pipelined as mvicp_optimize: the next evaluation is enqueued before the host learns whether the last one finished the
+  // solve; the kernels read what to evaluate (build or trial) from the state, and exit at once after termination
+  const int64_t max_evals = (int64_t)opt.max_calls * opt.iterations_per_call * (opt.max_trials + 1) + 2;
+  for (int i = 0; i < 8; ++i) c->h_flag[i] = 0;
+  c->eval_ev_used = 0;
+  int64_t issued = 0, seen = 0;
+  const double eps = opt.information_eps;
+  auto issue = [&]() -> int {
+    if ((int)c->eval_ev.size() < c->eval_ev_used + 2) { cudaEvent_t a, b; CU(cudaEventCreate(&a)); CU(cudaEventCreate(&b)); c->eval_ev.push_back(a); c->eval_ev.push_back(b); }
+    CU(cudaEventRecord(c->eval_ev[c->eval_ev_used], c->stream));
+    if (c->f32) launch_g2o_eval<true>(c, cost, nt, dS, eps); else launch_g2o_eval<false>(c, cost, nt, dS, eps);
+    CU(cudaEventRecord(c->eval_ev[c->eval_ev_used + 1], c->stream));
+    c->eval_ev_used += 2;
+    g2o_edge_kernel<<<E, EDGE_THREADS, 0, c->stream>>>(c->d_g2o_tile_begin.as<int32_t>(), c->d_partial.as<double>(), dS, c->d_eout.as<double>());
+    w.seq = (int32_t)(issued + 1);
+    g2o_step_kernel<<<1, STEP_THREADS, dyn, c->stream>>>(w);
+    c->stats.kernel_launches += 3;
+    ++issued;
+    return MVICP_OK;
+  };
+  RET(issue());
+  while (true) {
+    if (issued - seen < 2 && issued <= max_evals) RET(issue());
+    const int32_t want = (int32_t)(seen + 1);
+    int32_t v;
+    long spins = 0;
+    while (((v = c->h_flag[want & 7]) >> 1) != want) {
+      if ((++spins & 0xfffff) == 0 && cudaStreamQuery(c->stream) != cudaErrorNotReady) {
+        v = c->h_flag[want & 7];
+        if ((v >> 1) != want) { CU(cudaGetLastError()); return fail(MVICP_ERR_CUDA, "g2o step %d never reported", want); }
+        break;
+      }
+    }
+    ++seen;
+    if ((v & 1) != 0 || seen > max_evals) break;
+  }
+  CU(cudaEventRecord(c->ev[4], c->stream));
+  CU(cudaMemcpyAsync(&st, dS, sizeof st, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(c->h_poses.data(), c->d_poses.p, sizeof(double) * 16 * M, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  CU(cudaGetLastError());
+  if (chi2_per_call) CU(cudaMemcpy(chi2_per_call, c->d_g2o_chi.p, sizeof(double) * (st.call + 1), cudaMemcpyDeviceToHost));
+  c->ev_lm = true;
+  c->last_lm_iters = 1 << 20;
+  c->g2o_trials = st.n_trace;
+  if (summary) {
+    summary->calls = st.call; summary->iterations = st.n_iters; summary->trials = st.n_trials; summary->accepted = st.n_accepted;
+    summary->evaluations = st.n_evals; summary->ended = st.ended; summary->last_call_end = st.last_call_end;
+    summary->chi2_initial = st.chi_initial; summary->chi2_final = st.last_chi;
+  }
+  if (!st.done) return fail(MVICP_ERR_STATE, "g2o solve did not terminate within %lld evaluations", (long long)max_evals);
+  return MVICP_OK;
+}
+
+int mvicp_pairwise_g2o(const mvicp_config* cfg, int32_t cost, const double* src, const double* dst, const double* nor, int64_t n,
+                       const mvicp_g2o_options* opt_in, double* pose16_out, mvicp_g2o_summary* summary) {
+  if (!src || !dst || n <= 0 || !pose16_out) return fail(MVICP_ERR_INVALID, "mvicp_pairwise_g2o: bad arguments");
+  if (cost != MVICP_COST_P2P && !nor) return fail(MVICP_ERR_INVALID, "mvicp_pairwise_g2o: point-to-plane needs dst normals");
+  mvicp_g2o_options opt;
+  if (opt_in) opt = *opt_in; else { mvicp_default_g2o_options(&opt); opt.iterations_per_call = 300; }   // optimize(300), icp-g2o.cpp:72,133
+  opt.max_calls = 1;
+  mvicp_ctx* c = nullptr;
+  RET(mvicp_create(cfg, &c));
+  // vertex 0 = dst (fixed at the identity), vertex 1 = src (from the identity); edge 1 -> 0 with identity matches
+  const double* pts[2] = {dst, src}; const double* nrs[2] = {nor, nor};   // src normals are never read
+  const int64_t np[2] = {n, n};
+  int rc = mvicp_set_frames(c, 2, pts, nor ? nrs : nullptr, np);
+  const int32_t es = 1, ed = 0;
+  if (rc == MVICP_OK) rc = mvicp_set_graph(c, 1, &es, &ed);
+  if (rc == MVICP_OK) {
+    std::vector<int32_t> id(n); std::iota(id.begin(), id.end(), 0);
+    rc = mvicp_set_edge(c, 0, id.data(), id.data(), n, 1.0f);
+  }
+  if (rc == MVICP_OK) rc = mvicp_optimize_g2o(c, cost, &opt, summary, nullptr);
+  std::vector<double> poses(32);
+  if (rc == MVICP_OK) rc = mvicp_get_poses(c, poses.data());
+  if (rc == MVICP_OK) std::memcpy(pose16_out, poses.data() + 16, sizeof(double) * 16);
+  const std::string keep = g_err;
+  mvicp_destroy(c);
+  g_err = keep;
+  return rc;
+}
+
+int mvicp_g2o_trace(mvicp_ctx* c, double* out5, int64_t capacity, int64_t* n_trials) {
+  if (!c || capacity < 0 || (capacity && !out5)) return fail(MVICP_ERR_INVALID, "mvicp_g2o_trace: bad arguments");
+  if (n_trials) *n_trials = c->g2o_trials;
+  const int64_t k = std::min<int64_t>(capacity, std::min<int64_t>(c->g2o_trials, G2O_TRACE_CAP));
+  if (k <= 0) return MVICP_OK;
+  CU(cudaSetDevice(c->device));
+  CU(cudaStreamSynchronize(c->stream));
+  CU(cudaMemcpy(out5, c->d_g2o_trace.p, sizeof(double) * 5 * (size_t)k, cudaMemcpyDeviceToHost));
+  return MVICP_OK;
 }
 
 // ---- closed-form pairwise solvers (SURVEY 8(f) row 4; icp-closedform.cpp:9-54) ------------------------------
