@@ -232,6 +232,39 @@ int mvicp_get_normals(mvicp_ctx* ctx, int32_t frame, double* nor_xyz, float* ela
 /* Frame::getNeighbours(i, k) for every point i of one frame (frame.cpp:208-242): nn_idx[i*k + j], ascending distance. */
 int mvicp_knn_self(mvicp_ctx* ctx, int32_t frame, int32_t k, int32_t* nn_idx);
 
+/* Frame::getClosestPoint for n queries at once (q_xyz: n x 3 doubles in the frame's local coordinates): idx[i] / d2[i] are
+ * bit for bit what mvicp_closest_point returns for query i (same fp32 screen, fp64 re-rank, lowest index on ties).  A query
+ * with a non-finite coordinate gets idx -1 and d2 NaN; n = 0 does nothing; idx and d2 are nullable.  Host memory: the queries
+ * go through the context's buffers and the call returns with the results in place. */
+int mvicp_closest_points(mvicp_ctx* ctx, int32_t frame, const double* q_xyz, int64_t n, int64_t* idx, double* d2);
+
+/* ---- device twins: the calls above whose per-point arrays are in device memory ---------------------------------------
+ * Each one returns the same bytes as its host-memory twin, with the same argument checks, state errors (MVICP_ERR_STATE) and
+ * sharding rules (a rank sees the edges it processes; the others' lists are empty).  Every array argument must be device or
+ * managed memory of the context's device (cudaPointerGetAttributes); anything else, a host pointer included, gives
+ * MVICP_ERR_INVALID before any work is done.  Reads and writes are ordered on the context's stream (mvicp_get_stream): a caller
+ * that produces inputs or consumes outputs on another stream orders it against that one.  mvicp_set_frames_device and
+ * mvicp_set_edge_device return only after the caller's arrays have been read; the others are stream-ordered only and do not
+ * wait for the device. */
+/* mvicp_set_frames with pts_xyz[f] / nor_xyz[f] in device memory (the pointer arrays and n_pts stay on the host).  The frames
+ * are copied device to device and built there; under MVICP_FLAG_HOST_BUILD they are staged to the host and built there. */
+int mvicp_set_frames_device(mvicp_ctx* ctx, int32_t n_frames, const double* const* pts_xyz, const double* const* nor_xyz,
+                            const int64_t* n_pts);
+/* mvicp_set_edge with first / second in device memory: the same range check (a bad index leaves the edge as it was), the
+ * whole edge reset to "no match", the last occurrence of a duplicated src index wins, count stored as given. */
+int mvicp_set_edge_device(mvicp_ctx* ctx, int32_t e, const int32_t* first, const int32_t* second, int64_t count, float weight);
+/* mvicp_get_all_edges into device memory: out_records (16-byte Correspondance records, nullable), offsets (int64, n_edges + 1)
+ * and weights (nullable).  No host synchronisation; for that reason, when out_records is given, capacity must be at least the
+ * sum of the src cloud sizes over the edges this context processes (MVICP_ERR_INVALID otherwise, before any launch).  Records
+ * past offsets[n_edges] are unspecified. */
+int mvicp_get_all_edges_device(mvicp_ctx* ctx, void* out_records, int64_t capacity, int64_t* offsets, float* weights);
+/* mvicp_closest_points with q_xyz, idx and d2 in device memory. */
+int mvicp_closest_points_device(mvicp_ctx* ctx, int32_t frame, const double* q_xyz, int64_t n, int64_t* idx, double* d2);
+/* mvicp_get_normals into device memory (N x 3 doubles). */
+int mvicp_get_normals_device(mvicp_ctx* ctx, int32_t frame, double* nor_xyz);
+/* mvicp_knn_self into device memory (N x k int32); scratch comes from the context's reusable buffers. */
+int mvicp_knn_self_device(mvicp_ctx* ctx, int32_t frame, int32_t k, int32_t* nn_idx);
+
 /* ---- multi-GPU: one process per GPU; the edges with a free src frame, in graph order, are cut into world_size
  * contiguous runs of equal query count (every rank holds all clouds and ends every call with identical poses) ---- */
 int mvicp_nccl_unique_id(void* out128);   /* rank 0 creates, the launcher broadcasts the 128 bytes */

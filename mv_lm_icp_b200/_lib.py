@@ -63,7 +63,9 @@ EXPORTS = ["mvicp_default_lm_options", "mvicp_last_error", "mvicp_create", "mvic
            "mvicp_correspond", "mvicp_get_edge", "mvicp_get_all_edges", "mvicp_get_nn", "mvicp_set_edge", "mvicp_closest_point",
            "mvicp_optimize", "mvicp_icp_round", "mvicp_pairwise", "mvicp_pairwise_closed", "mvicp_recompute_normals", "mvicp_get_normals", "mvicp_knn_self", "mvicp_nccl_unique_id", "mvicp_comm_init",
            "mvicp_get_stats", "mvicp_get_stream", "mvicp_sync", "mvicp_abi_version", "mvicp_host_alloc", "mvicp_host_free",
-           "mvicp_default_g2o_options", "mvicp_optimize_g2o", "mvicp_pairwise_g2o", "mvicp_g2o_trace"]
+           "mvicp_default_g2o_options", "mvicp_optimize_g2o", "mvicp_pairwise_g2o", "mvicp_g2o_trace",
+           "mvicp_closest_points", "mvicp_set_frames_device", "mvicp_set_edge_device", "mvicp_get_all_edges_device",
+           "mvicp_closest_points_device", "mvicp_get_normals_device", "mvicp_knn_self_device"]
 
 
 def build(force=False):

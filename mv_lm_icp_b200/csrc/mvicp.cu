@@ -24,6 +24,7 @@
 #include "../../include/mvicp.h"
 #include "closed.cuh"
 #include "compact.cuh"
+#include "device_io.cuh"
 #include "far.cuh"
 #include "g2o.cuh"
 #include "knn.cuh"
@@ -131,6 +132,10 @@ struct mvicp_ctx {
   int eval_ev_used = 0;
   bool ev_knn = false, ev_lm = false;
   float lm_eval_acc = 0.f;
+  // scratch of the device twins (mvicp_closest_points, mvicp_set_edge_device, mvicp_knn_self_device)
+  DevBuf d_cpq, d_cpr;         // queries, then results (int64 index | fp64 d2)
+  DevBuf d_set_win, d_set_bad; // winning position + 1 per src slot, lowest bad position
+  DevBuf d_knn_nor;            // the normals the k-NN kernel also writes
 };
 
 static inline int owner_of(const mvicp_ctx* c, int frame) { return (int)(((int64_t)frame * c->world) / std::max(1, c->M)); }
@@ -263,7 +268,9 @@ static int build_frames_on_device(mvicp_ctx* c, int M, const std::vector<double*
   return MVICP_OK;
 }
 
-static int set_frames_device(mvicp_ctx* c, int M, const double* const* pts, const double* const* nor, const int64_t* n_pts) {
+// kind: cudaMemcpyHostToDevice (mvicp_set_frames) or cudaMemcpyDeviceToDevice (mvicp_set_frames_device)
+static int set_frames_device(mvicp_ctx* c, int M, const double* const* pts, const double* const* nor, const int64_t* n_pts,
+                             cudaMemcpyKind kind) {
   std::vector<double*> d_xyz(M, nullptr), d_nor(M, nullptr);
   int* d_flags = nullptr;
   auto cleanup = [&]() { for (double* p : d_xyz) cudaFree(p); for (double* p : d_nor) cudaFree(p); cudaFree(d_flags); };
@@ -274,11 +281,11 @@ static int set_frames_device(mvicp_ctx* c, int M, const double* const* pts, cons
   for (int f = 0; f < M && err == cudaSuccess; ++f) {
     const size_t bytes = sizeof(double) * 3 * (size_t)n_pts[f];
     err = cudaMalloc(&d_xyz[f], bytes);
-    if (err == cudaSuccess) err = cudaMemcpyAsync(d_xyz[f], pts[f], bytes, cudaMemcpyHostToDevice, c->stream);
+    if (err == cudaSuccess) err = cudaMemcpyAsync(d_xyz[f], pts[f], bytes, kind, c->stream);
     if (err == cudaSuccess) kd_scan_kernel<<<2 * NUM_SMS, 256, 0, c->stream>>>(d_xyz[f], 3ll * n_pts[f], d_flags + 4 * f);
     if (err == cudaSuccess && nor && nor[f]) {
       err = cudaMalloc(&d_nor[f], bytes);
-      if (err == cudaSuccess) err = cudaMemcpyAsync(d_nor[f], nor[f], bytes, cudaMemcpyHostToDevice, c->stream);
+      if (err == cudaSuccess) err = cudaMemcpyAsync(d_nor[f], nor[f], bytes, kind, c->stream);
       if (err == cudaSuccess) kd_scan_kernel<<<2 * NUM_SMS, 256, 0, c->stream>>>(d_nor[f], 3ll * n_pts[f], d_flags + 4 * f + 2);
     }
     c->stats.kernel_launches += (nor && nor[f]) ? 2 : 1;
@@ -328,6 +335,17 @@ static void pad_records(bool f32, void* recs, int64_t n, int64_t n_pad) {
     if (f32) { float4 r; r.x = r.y = r.z = INFINITY; std::memcpy(&r.w, &w, 4); reinterpret_cast<float4*>(recs)[i] = r; }
     else { double4a r; r.x = r.y = r.z = INFINITY; const long long wl = w; std::memcpy(&r.w, &wl, 8); reinterpret_cast<double4a*>(recs)[i] = r; }
   }
+}
+
+// Arguments of the `_device` entry points: device (or managed) memory of the context's device, nothing else -- a host pointer
+// is refused before any work is done.
+static int check_device_ptr(const mvicp_ctx* c, const void* p, const char* fn, const char* what) {
+  if (!p) return fail(MVICP_ERR_INVALID, "%s: %s is null", fn, what);
+  cudaPointerAttributes a; std::memset(&a, 0, sizeof a);
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return fail(MVICP_ERR_INVALID, "%s: %s is not device memory", fn, what); }
+  if ((a.type != cudaMemoryTypeDevice && a.type != cudaMemoryTypeManaged) || a.device != c->device)
+    return fail(MVICP_ERR_INVALID, "%s: %s is not device memory of device %d", fn, what, c->device);
+  return MVICP_OK;
 }
 
 // =================================================================================================
@@ -386,6 +404,7 @@ void mvicp_destroy(mvicp_ctx* c) {
                     &c->d_gc, &c->d_scale, &c->d_diag, &c->d_L, &c->d_rhs, &c->d_step, &c->d_eout,
                     &c->d_hb_ptr, &c->d_hb_row, &c->d_hb_col, &c->d_hc_edge, &c->d_hc_sub, &c->d_gb_ptr, &c->d_gc_edge,
                     &c->d_gc_side, &c->d_posegather, &c->d_rlast, &c->d_rfirst, &c->d_rowbase, &c->d_gen, &c->d_obb, &c->d_single, &c->d_prof, &c->d_tile_count, &c->d_tile_off, &c->d_edge_off, &c->d_recs,
+                    &c->d_cpq, &c->d_cpr, &c->d_set_win, &c->d_set_bad, &c->d_knn_nor,
                     &c->d_g2o_state, &c->d_g2o_x, &c->d_g2o_ev, &c->d_g2o_nop, &c->d_g2o_chi, &c->d_g2o_trace, &c->d_g2o_tiles,
                     &c->d_g2o_tile_begin, &c->d_g2o_cnt};
   for (DevBuf* b : bufs) b->release();
@@ -398,7 +417,9 @@ void mvicp_destroy(mvicp_ctx* c) {
   delete c;
 }
 
-int mvicp_set_frames(mvicp_ctx* c, int32_t M, const double* const* pts, const double* const* nor, const int64_t* n_pts) {
+}  // extern "C"
+// mvicp_set_frames and its device twin: dev_src = the coordinate arrays are device memory (checked by the caller)
+static int set_frames_impl(mvicp_ctx* c, int32_t M, const double* const* pts, const double* const* nor, const int64_t* n_pts, bool dev_src) {
   if (!c || M <= 0 || !pts || !n_pts) return fail(MVICP_ERR_INVALID, "mvicp_set_frames: bad arguments");
   CU(cudaSetDevice(c->device));
   CU(cudaStreamSynchronize(c->stream));
@@ -416,8 +437,31 @@ int mvicp_set_frames(mvicp_ctx* c, int32_t M, const double* const* pts, const do
   c->nor_dbl.clear();
   c->obb_ready = false;
 #ifdef __CUDACC__
-  if (!(c->flags & MVICP_FLAG_HOST_BUILD)) { RET(set_frames_device(c, M, pts, nor, n_pts)); return finish_set_frames(c, M); }
+  if (!(c->flags & MVICP_FLAG_HOST_BUILD)) {
+    RET(set_frames_device(c, M, pts, nor, n_pts, dev_src ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice));
+    return finish_set_frames(c, M);
+  }
 #endif
+  // the host build of device-resident frames: stage them to the host first (the A/B flag and the host model take this path)
+  std::vector<std::vector<double>> staged;
+  std::vector<const double*> hp, hn;
+  if (dev_src) {
+    staged.resize(2 * (size_t)M); hp.assign(M, nullptr); hn.assign(M, nullptr);
+    for (int f = 0; f < M; ++f) {
+      const size_t cnt = 3 * (size_t)n_pts[f];
+      staged[2 * f].resize(cnt);
+      CU(cudaMemcpyAsync(staged[2 * f].data(), pts[f], sizeof(double) * cnt, cudaMemcpyDeviceToHost, c->stream));
+      hp[f] = staged[2 * f].data();
+      if (nor && nor[f]) {
+        staged[2 * f + 1].resize(cnt);
+        CU(cudaMemcpyAsync(staged[2 * f + 1].data(), nor[f], sizeof(double) * cnt, cudaMemcpyDeviceToHost, c->stream));
+        hn[f] = staged[2 * f + 1].data();
+      }
+    }
+    CU(cudaStreamSynchronize(c->stream));
+    pts = hp.data();
+    if (nor) nor = hn.data();
+  }
   for (int f = 0; f < M; ++f) f32 = f32 && all_fp32(pts[f], 3 * n_pts[f]) && (!nor || !nor[f] || all_fp32(nor[f], 3 * n_pts[f]));
   c->f32 = f32; c->nor_f32 = f32;
   const size_t rec = f32 ? sizeof(float4) : sizeof(double4a);
@@ -492,6 +536,22 @@ int mvicp_set_frames(mvicp_ctx* c, int32_t M, const double* const* pts, const do
     c->obb_ready = true;
   }
   return finish_set_frames(c, M);
+}
+extern "C" {
+
+int mvicp_set_frames(mvicp_ctx* c, int32_t M, const double* const* pts, const double* const* nor, const int64_t* n_pts) {
+  return set_frames_impl(c, M, pts, nor, n_pts, false);
+}
+
+int mvicp_set_frames_device(mvicp_ctx* c, int32_t M, const double* const* pts, const double* const* nor, const int64_t* n_pts) {
+  if (!c || M <= 0 || !pts || !n_pts) return fail(MVICP_ERR_INVALID, "mvicp_set_frames_device: bad arguments");
+  CU(cudaSetDevice(c->device));
+  for (int f = 0; f < M; ++f) {
+    if (n_pts[f] <= 0 || !pts[f]) continue;   // the twin's own checks report these
+    RET(check_device_ptr(c, pts[f], "mvicp_set_frames_device", "pts_xyz[f]"));
+    if (nor && nor[f]) RET(check_device_ptr(c, nor[f], "mvicp_set_frames_device", "nor_xyz[f]"));
+  }
+  return set_frames_impl(c, M, pts, nor, n_pts, true);
 }
 
 int mvicp_set_poses(mvicp_ctx* c, const double* poses16, const uint8_t* fixed) {
@@ -797,10 +857,8 @@ int mvicp_get_edge(mvicp_ctx* c, int32_t e, int32_t* first, int32_t* second, dou
   return MVICP_OK;
 }
 
-int mvicp_get_all_edges(mvicp_ctx* c, void* out_records, int64_t capacity, int64_t* offsets, float* weights) {
-  if (!c || !c->E || !offsets) return fail(MVICP_ERR_INVALID, "mvicp_get_all_edges: bad arguments / no graph");
-  if (!c->have_corr) return fail(MVICP_ERR_STATE, "mvicp_get_all_edges: call mvicp_correspond first");
-  CU(cudaSetDevice(c->device));
+// inliers per tile and their exclusive scan: d_tile_off (first record of every tile), d_edge_off (of every edge, [E] = total)
+static int compact_count_scan(mvicp_ctx* c) {
   const int E = c->E, nt = c->n_knn_tiles;
   RET(c->d_tile_count.reserve(sizeof(unsigned int) * std::max(1, nt)));
   RET(c->d_tile_off.reserve(sizeof(unsigned long long) * std::max(1, nt)));
@@ -809,6 +867,15 @@ int mvicp_get_all_edges(mvicp_ctx* c, void* out_records, int64_t capacity, int64
   compact_scan_kernel<<<1, 1024, 0, c->stream>>>(c->d_tile_count.as<unsigned int>(), nt, c->d_knn_tiles.as<Tile>(), E,
                                                  c->d_tile_off.as<unsigned long long>(), c->d_edge_off.as<unsigned long long>());
   c->stats.kernel_launches += nt ? 2 : 1;
+  return MVICP_OK;
+}
+
+int mvicp_get_all_edges(mvicp_ctx* c, void* out_records, int64_t capacity, int64_t* offsets, float* weights) {
+  if (!c || !c->E || !offsets) return fail(MVICP_ERR_INVALID, "mvicp_get_all_edges: bad arguments / no graph");
+  if (!c->have_corr) return fail(MVICP_ERR_STATE, "mvicp_get_all_edges: call mvicp_correspond first");
+  CU(cudaSetDevice(c->device));
+  const int E = c->E, nt = c->n_knn_tiles;
+  RET(compact_count_scan(c));
   std::vector<unsigned long long> eo(E + 1);
   CU(cudaMemcpyAsync(eo.data(), c->d_edge_off.p, sizeof(unsigned long long) * (E + 1), cudaMemcpyDeviceToHost, c->stream));
   if (weights) CU(cudaMemcpyAsync(weights, c->d_weight.p, sizeof(float) * E, cudaMemcpyDeviceToHost, c->stream));
@@ -825,6 +892,35 @@ int mvicp_get_all_edges(mvicp_ctx* c, void* out_records, int64_t capacity, int64
       CU(cudaMemcpyAsync(out_records, c->d_recs.p, sizeof(CorrRec) * (size_t)total, cudaMemcpyDeviceToHost, c->stream));
       CU(cudaStreamSynchronize(c->stream));
     }
+  }
+  CU(cudaGetLastError());
+  return MVICP_OK;
+}
+
+// The same three compaction kernels, writing straight into the caller's device buffer; offsets and weights are device-to-device
+// copies.  Nothing waits for the device: the capacity is checked up front against what the kernels may write at most.
+int mvicp_get_all_edges_device(mvicp_ctx* c, void* out_records, int64_t capacity, int64_t* offsets, float* weights) {
+  if (!c || !c->E || !offsets) return fail(MVICP_ERR_INVALID, "mvicp_get_all_edges_device: bad arguments / no graph");
+  if (!c->have_corr) return fail(MVICP_ERR_STATE, "mvicp_get_all_edges_device: call mvicp_correspond first");
+  CU(cudaSetDevice(c->device));
+  RET(check_device_ptr(c, offsets, "mvicp_get_all_edges_device", "offsets"));
+  if (out_records) RET(check_device_ptr(c, out_records, "mvicp_get_all_edges_device", "out_records"));
+  if (weights) RET(check_device_ptr(c, weights, "mvicp_get_all_edges_device", "weights"));
+  const int E = c->E, nt = c->n_knn_tiles;
+  if (out_records) {
+    int64_t bound = 0;
+    for (const EdgeDev& ed : c->h_edges) if (ed.owned) bound += ed.n_src;
+    if (capacity < bound)
+      return fail(MVICP_ERR_INVALID, "mvicp_get_all_edges_device: up to %lld records, capacity %lld", (long long)bound, (long long)capacity);
+  }
+  RET(compact_count_scan(c));
+  static_assert(sizeof(unsigned long long) == sizeof(int64_t), "offsets are copied as they are");
+  CU(cudaMemcpyAsync(offsets, c->d_edge_off.p, sizeof(int64_t) * (E + 1), cudaMemcpyDeviceToDevice, c->stream));
+  if (weights) CU(cudaMemcpyAsync(weights, c->d_weight.p, sizeof(float) * E, cudaMemcpyDeviceToDevice, c->stream));
+  if (out_records && nt) {
+    compact_scatter_kernel<<<nt, KNN_TILE, 0, c->stream>>>(c->d_edges.as<EdgeDev>(), c->d_knn_tiles.as<Tile>(), c->d_corr.as<int32_t>(), c->d_d2.as<double>(),
+                                                           c->d_tile_off.as<unsigned long long>(), reinterpret_cast<CorrRec*>(out_records));
+    c->stats.kernel_launches += 1;
   }
   CU(cudaGetLastError());
   return MVICP_OK;
@@ -875,6 +971,41 @@ int mvicp_set_edge(mvicp_ctx* c, int32_t e, const int32_t* first, const int32_t*
   return MVICP_OK;
 }
 
+// mvicp_set_edge with first / second in device memory: range check + last-occurrence winner per slot, then the write, which the
+// device skips when the check failed; one readback of the check, after which the caller's arrays have been read
+int mvicp_set_edge_device(mvicp_ctx* c, int32_t e, const int32_t* first, const int32_t* second, int64_t count, float weight) {
+  if (!c || e < 0 || e >= c->E || count < 0 || (count && (!first || !second))) return fail(MVICP_ERR_INVALID, "mvicp_set_edge_device: bad arguments");
+  CU(cudaSetDevice(c->device));
+  if (count) {
+    RET(check_device_ptr(c, first, "mvicp_set_edge_device", "first"));
+    RET(check_device_ptr(c, second, "mvicp_set_edge_device", "second"));
+  }
+  const EdgeDev& ed = c->h_edges[e];
+  const int n_dst = (int)c->n_pts[ed.dst];
+  RET(c->d_set_win.reserve(sizeof(unsigned long long) * (size_t)std::max(1, ed.n_src)));
+  RET(c->d_set_bad.reserve(sizeof(unsigned long long)));
+  unsigned long long* win = c->d_set_win.as<unsigned long long>();
+  unsigned long long* bad = c->d_set_bad.as<unsigned long long>();
+  CU(cudaMemsetAsync(win, 0, sizeof(unsigned long long) * (size_t)ed.n_src, c->stream));
+  CU(cudaMemsetAsync(bad, 0xff, sizeof(unsigned long long), c->stream));
+  if (count) {
+    const int grid = (int)std::min<int64_t>((count + 255) / 256, 8 * NUM_SMS);
+    set_edge_scan_kernel<<<grid, 256, 0, c->stream>>>(first, second, (long long)count, ed.n_src, n_dst, win, bad);
+    c->stats.kernel_launches += 1;
+  }
+  const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((ed.n_src + 255) / 256, 8 * NUM_SMS));
+  set_edge_write_kernel<<<grid, 256, 0, c->stream>>>(second, win, ed.n_src, bad, c->d_corr.as<int32_t>() + ed.off, c->d_weight.as<float>() + e,
+                                                     c->d_count.as<unsigned long long>() + e, weight, (unsigned long long)count);
+  c->stats.kernel_launches += 1;
+  unsigned long long h_bad = 0;
+  CU(cudaMemcpyAsync(&h_bad, bad, sizeof h_bad, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  CU(cudaGetLastError());
+  if (h_bad != ~0ull) return fail(MVICP_ERR_INVALID, "mvicp_set_edge_device: index out of range at %lld", (long long)h_bad);
+  c->cert_valid = false;   // as mvicp_set_edge
+  return MVICP_OK;
+}
+
 int mvicp_closest_point(mvicp_ctx* c, int32_t frame, const double q[3], int64_t* idx, double* d2) {
   if (!c || frame < 0 || frame >= c->M || !q) return fail(MVICP_ERR_INVALID, "mvicp_closest_point: bad arguments");
   CU(cudaSetDevice(c->device));
@@ -889,6 +1020,43 @@ int mvicp_closest_point(mvicp_ctx* c, int32_t frame, const double q[3], int64_t*
   if (idx) *idx = hi;
   if (d2) *d2 = hd;
   return MVICP_OK;
+}
+
+}  // extern "C"
+static int launch_closest_points(mvicp_ctx* c, int frame, const double* q, int64_t n, long long* idx, double* d2) {
+  const int grid = (int)std::min<int64_t>((n + 127) / 128, 64 * NUM_SMS);
+  if (c->f32) closest_points_kernel<true><<<grid, 128, 0, c->stream>>>(c->d_frames.as<FrameDev>(), frame, q, (long long)n, idx, d2);
+  else closest_points_kernel<false><<<grid, 128, 0, c->stream>>>(c->d_frames.as<FrameDev>(), frame, q, (long long)n, idx, d2);
+  c->stats.kernel_launches += 1;
+  CU(cudaGetLastError());
+  return MVICP_OK;
+}
+extern "C" {
+
+// mvicp_closest_point for n queries at once: the queries go up through the context's buffers, the results come back
+int mvicp_closest_points(mvicp_ctx* c, int32_t frame, const double* q, int64_t n, int64_t* idx, double* d2) {
+  if (!c || frame < 0 || frame >= c->M || n < 0 || (n && !q)) return fail(MVICP_ERR_INVALID, "mvicp_closest_points: bad arguments");
+  if (!n) return MVICP_OK;
+  CU(cudaSetDevice(c->device));
+  RET(c->d_cpq.reserve(sizeof(double) * 3 * (size_t)n));
+  RET(c->d_cpr.reserve(16 * (size_t)n));
+  long long* d_i = c->d_cpr.as<long long>(); double* d_d = c->d_cpr.as<double>() + n;
+  CU(cudaMemcpyAsync(c->d_cpq.p, q, sizeof(double) * 3 * (size_t)n, cudaMemcpyHostToDevice, c->stream));
+  RET(launch_closest_points(c, frame, c->d_cpq.as<double>(), n, d_i, d_d));
+  if (idx) CU(cudaMemcpyAsync(idx, d_i, sizeof(int64_t) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+  if (d2) CU(cudaMemcpyAsync(d2, d_d, sizeof(double) * (size_t)n, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  return MVICP_OK;
+}
+
+int mvicp_closest_points_device(mvicp_ctx* c, int32_t frame, const double* q, int64_t n, int64_t* idx, double* d2) {
+  if (!c || frame < 0 || frame >= c->M || n < 0 || (n && !q)) return fail(MVICP_ERR_INVALID, "mvicp_closest_points_device: bad arguments");
+  if (!n) return MVICP_OK;
+  CU(cudaSetDevice(c->device));
+  RET(check_device_ptr(c, q, "mvicp_closest_points_device", "q_xyz"));
+  if (idx) RET(check_device_ptr(c, idx, "mvicp_closest_points_device", "idx"));
+  if (d2) RET(check_device_ptr(c, d2, "mvicp_closest_points_device", "d2"));
+  return launch_closest_points(c, frame, q, n, reinterpret_cast<long long*>(idx), d2);
 }
 
 // ---- LM ------------------------------------------------------------------------------------------
@@ -1575,6 +1743,29 @@ int mvicp_knn_self(mvicp_ctx* c, int32_t frame, int32_t k, int32_t* nn_idx) {
   CU(cudaMemcpyAsync(nn_idx, d_nn, sizeof(int32_t) * (size_t)k * n, cudaMemcpyDeviceToHost, c->stream));
   CU(cudaStreamSynchronize(c->stream));
   cudaFree(d_nor); cudaFree(d_nn);
+  CU(cudaGetLastError());
+  return MVICP_OK;
+}
+
+int mvicp_get_normals_device(mvicp_ctx* c, int32_t frame, double* nor_xyz) {
+  if (!c || frame < 0 || frame >= c->M || !nor_xyz) return fail(MVICP_ERR_INVALID, "mvicp_get_normals_device: bad arguments");
+  if ((int)c->nor_dbl.size() <= frame || !c->nor_dbl[frame]) return fail(MVICP_ERR_STATE, "mvicp_get_normals_device: call mvicp_recompute_normals first");
+  CU(cudaSetDevice(c->device));
+  RET(check_device_ptr(c, nor_xyz, "mvicp_get_normals_device", "nor_xyz"));
+  CU(cudaMemcpyAsync(nor_xyz, c->nor_dbl[frame], sizeof(double) * 3 * (size_t)c->n_pts[frame], cudaMemcpyDeviceToDevice, c->stream));
+  return MVICP_OK;
+}
+
+// mvicp_knn_self into the caller's device buffer; the normals the kernel computes on the way go to a reusable context buffer
+int mvicp_knn_self_device(mvicp_ctx* c, int32_t frame, int32_t k, int32_t* nn_idx) {
+  if (!c || frame < 0 || frame >= c->M || !nn_idx || k < 1 || k > KNN_MAXK) return fail(MVICP_ERR_INVALID, "mvicp_knn_self_device: bad arguments");
+  CU(cudaSetDevice(c->device));
+  RET(check_device_ptr(c, nn_idx, "mvicp_knn_self_device", "nn_idx"));
+  const int n = (int)c->n_pts[frame];
+  RET(c->d_knn_nor.reserve(sizeof(double) * 3 * (size_t)n));
+  if (c->f32) normals_kernel<true><<<(n + 127) / 128, 128, 0, c->stream>>>(c->d_frames.as<FrameDev>(), frame, k, c->d_knn_nor.as<double>(), nn_idx);
+  else normals_kernel<false><<<(n + 127) / 128, 128, 0, c->stream>>>(c->d_frames.as<FrameDev>(), frame, k, c->d_knn_nor.as<double>(), nn_idx);
+  c->stats.kernel_launches += 1;
   CU(cudaGetLastError());
   return MVICP_OK;
 }

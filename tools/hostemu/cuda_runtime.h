@@ -190,6 +190,8 @@ inline int __ffs(unsigned x) { return __builtin_ffs((int)x); }
 inline uint2 make_uint2(unsigned x, unsigned y) { uint2 r; r.x = x; r.y = y; return r; }
 template <class T> inline T atomicAdd(T* p, T v) { const T o = *p; *p = o + v; return o; }
 template <class T> inline T atomicExch(T* p, T v) { const T o = *p; *p = v; return o; }
+template <class T> inline T atomicMin(T* p, T v) { const T o = *p; if (v < o) *p = v; return o; }
+template <class T> inline T atomicMax(T* p, T v) { const T o = *p; if (v > o) *p = v; return o; }
 inline void __threadfence() {} inline void __threadfence_system() {} inline void __threadfence_block() {}
 inline long long clock64() { return std::chrono::steady_clock::now().time_since_epoch().count(); }
 
@@ -253,3 +255,12 @@ template <class K> inline cudaError_t cudaFuncSetAttribute(K, int, int) { return
 inline cudaError_t cudaIpcGetMemHandle(cudaIpcMemHandle_t*, void*) { return cudaErrorNotSupported; }
 inline cudaError_t cudaIpcOpenMemHandle(void**, cudaIpcMemHandle_t, unsigned) { return cudaErrorNotSupported; }
 inline cudaError_t cudaIpcCloseMemHandle(void*) { return cudaSuccess; }
+// every allocation is host memory here, and all of it stands for device memory of device 0: the `_device` entry points accept
+// numpy buffers on this model (a null pointer is unregistered, as on the device)
+enum cudaMemoryType { cudaMemoryTypeUnregistered = 0, cudaMemoryTypeHost = 1, cudaMemoryTypeDevice = 2, cudaMemoryTypeManaged = 3 };
+struct cudaPointerAttributes { cudaMemoryType type; int device; void* devicePointer; void* hostPointer; };
+inline cudaError_t cudaPointerGetAttributes(cudaPointerAttributes* a, const void* p) {
+  a->type = p ? cudaMemoryTypeDevice : cudaMemoryTypeUnregistered; a->device = 0;
+  a->devicePointer = const_cast<void*>(p); a->hostPointer = nullptr;
+  return cudaSuccess;
+}
