@@ -210,26 +210,19 @@ __global__ void g2o_count_kernel(const EdgeDev* __restrict__ edges, const Tile* 
 struct G2oWork {
   G2oState* S;
   const double* eout;            // [E][EOUT] from g2o_edge_kernel
-  volatile int32_t* host_flag;   // mapped pinned ring: (sequence << 1) | done
-  int32_t seq;
   Rt* x;                         // [M] current estimate of every vertex
   Rt* ev;                        // [M] evaluation point: x (build) or the trial estimate
   int32_t* n_oplus;              // [M] VertexSE3::_numOplusCalls
-  const int32_t* col;            // [M] first column or -1 (fixed, or no correspondence)
-  const int32_t* hb_ptr; const int32_t* hb_row; const int32_t* hb_col; const int32_t* hc_edge; const int32_t* hc_sub; int32_t n_hblocks;
-  const int32_t* gb_ptr; const int32_t* gc_edge; const int32_t* gc_side;
-  const int32_t* rlast; const int32_t* rfirst; const int32_t* rowbase;
-  double *H, *b, *Lg, *rhs;
-  double* poses16;
+  NormalLayout lay;              // a frame has a column when it is free and has a correspondence
+  double *H, *g;                 // g = sum J^T Omega e: g2o's b is -g
   double* chi_calls;             // [max_calls + 1]: chi2 before the first call, then after every call
   double* trace;                 // [trace_cap][5]: lambda, chi, tchi, rho, accepted -- one row per trial
-  int32_t l_in_smem;
 };
 
 __global__ void g2o_init_kernel(G2oWork w, int M) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= M) return;
-  Rt a; pose16_to_Rt(w.poses16 + 16 * f, &a);
+  Rt a; pose16_to_Rt(w.lay.poses16 + 16 * f, &a);
   w.x[f] = a; w.ev[f] = a; w.n_oplus[f] = 0;
 }
 
@@ -266,20 +259,17 @@ __global__ void __launch_bounds__(STEP_THREADS) g2o_step_kernel(G2oWork w) {
   __shared__ double red[40];
   __shared__ G2oState s_state;
   __shared__ int s_solve, s_accept, s_tobuild;
-  if (w.S->done) { if (threadIdx.x == 0) { w.host_flag[w.seq & 7] = (w.seq << 1) | 1; __threadfence_system(); } return; }
+  if (w.S->done) { if (threadIdx.x == 0) publish_step(w.lay, true); return; }
   const int tid = threadIdx.x, T = blockDim.x;
-  for (int i = tid; i < (int)(sizeof(G2oState) / sizeof(int32_t)); i += T)
-    reinterpret_cast<int32_t*>(&s_state)[i] = reinterpret_cast<const int32_t*>(w.S)[i];
-  __syncthreads();
+  copy_state(&s_state, w.S);
   G2oState* S = &s_state;
   const int n = S->n, M = S->M, E = S->E;
   const int phase = S->phase;   // thread 0 moves S->phase on below
+  const NormalLayout& lay = w.lay;
   double* colj = smem; double* dg = smem + 2 * (n + 1);
-  double* L = w.l_in_smem ? smem + 3 * (n + 1) : w.Lg;
+  double* L = lay.l_in_smem ? smem + 3 * (n + 1) : lay.Lg;
 
-  double chi_eval = 0.0;   // edges summed in a fixed order
-  for (int e = tid; e < E; e += T) chi_eval += w.eout[(size_t)EOUT * e + 156];
-  chi_eval = block_sum(chi_eval, red);
+  const double chi_eval = edge_cost_sum(w.eout, E, red);
 
   // end of an iteration (Terminate: trials exhausted or rho == 0), of a call (SparseOptimizer::optimize), of the outer loop
   auto end_iter = [&](double rho) {   // thread 0 only
@@ -309,23 +299,9 @@ __global__ void __launch_bounds__(STEP_THREADS) g2o_step_kernel(G2oWork w) {
 
   if (tid == 0) { s_solve = 0; s_accept = 0; s_tobuild = 0; S->n_evals += 1; }
   if (phase == G2O_BUILD) {
-    // H = sum J^T Omega J over the listed blocks, b = -sum J^T Omega e
-    for (int idx = tid; idx < w.n_hblocks * 36; idx += T) {
-      const int bk = idx / 36, r = idx - 36 * bk, i = r / 6, j = r - 6 * i;
-      double s = 0;
-      for (int c = w.hb_ptr[bk]; c < w.hb_ptr[bk + 1]; ++c) {
-        const int e = w.hc_edge[c], sub = w.hc_sub[c];   // sub: 0 ss, 1 sk, 2 ks, 3 kk
-        s += w.eout[(size_t)EOUT * e + (6 * (sub >> 1) + i) * 12 + 6 * (sub & 1) + j];
-      }
-      w.H[(size_t)(w.hb_row[bk] + i) * n + w.hb_col[bk] + j] = s;
-    }
-    for (int idx = tid; idx < M * 6; idx += T) {
-      const int f = idx / 6, i = idx - 6 * f;
-      if (w.col[f] < 0) continue;
-      double s = 0;
-      for (int c = w.gb_ptr[f]; c < w.gb_ptr[f + 1]; ++c) s += w.eout[(size_t)EOUT * w.gc_edge[c] + 144 + 6 * w.gc_side[c] + i];
-      w.b[w.col[f] + i] = -s;
-    }
+    // H = sum J^T Omega J over the listed blocks, g = sum J^T Omega e
+    gather_blocks(lay, w.eout, n, w.H);
+    gather_gradient(lay, w.eout, M, w.g);
     __syncthreads();
     double md = 0.0;
     for (int j = tid; j < n; j += T) md = fmax(md, fabs(w.H[(size_t)j * n + j]));
@@ -356,28 +332,28 @@ __global__ void __launch_bounds__(STEP_THREADS) g2o_step_kernel(G2oWork w) {
   __syncthreads();
 
   while (s_solve) {
-    // (H + lambda I) dx = b, skyline Cholesky of lm_step.cuh
+    // (H + lambda I) dx = b = -g, skyline Cholesky of lm_step.cuh
     const double lambda = S->lambda;
     for (int i = tid >> 5; i < n; i += T >> 5) {
-      const int rbi = w.rowbase[i];
-      for (int j = w.rfirst[i] + (tid & 31); j <= i; j += 32) L[rbi + j] = w.H[(size_t)i * n + j] + (i == j ? lambda : 0.0);
+      const int rbi = lay.rowbase[i];
+      for (int j = lay.rfirst[i] + (tid & 31); j <= i; j += 32) L[rbi + j] = w.H[(size_t)i * n + j] + (i == j ? lambda : 0.0);
     }
-    { const int rbn = w.rowbase[n]; for (int j = tid; j < n; j += T) L[rbn + j] = w.b[j]; }
+    { const int rbn = lay.rowbase[n]; for (int j = tid; j < n; j += T) L[rbn + j] = -w.g[j]; }
     __syncthreads();
-    bool ok = chol_solve(L, w.rowbase, n, colj, dg, w.rhs, w.rlast, w.rfirst);
+    bool ok = chol_solve(L, lay.rowbase, n, colj, dg, lay.rhs, lay.rlast, lay.rfirst);
     double bad = 0.0;
-    if (ok) for (int j = tid; j < n; j += T) if (!isfinite(w.rhs[j])) bad = 1.0;
+    if (ok) for (int j = tid; j < n; j += T) if (!isfinite(lay.rhs[j])) bad = 1.0;
     bad = block_sum(bad, red);
     ok = ok && bad == 0.0;
     double sc = 0.0;
-    if (ok) for (int j = tid; j < n; j += T) sc += w.rhs[j] * (lambda * w.rhs[j] + w.b[j]);
+    if (ok) for (int j = tid; j < n; j += T) sc += lay.rhs[j] * (lambda * lay.rhs[j] - w.g[j]);
     sc = block_sum(sc, red);   // computeScale()
     // the update is applied to every vertex in the problem (and counted) even when the factorisation failed; it is undone then
     for (int f = tid; f < M; f += T) {
-      const int cf = w.col[f];
+      const int cf = lay.col[f];
       if (cf < 0) continue;
       Rt nx;
-      g2o_oplus(w.x[f], w.rhs + cf, &w.n_oplus[f], S->ortho_after, &nx);
+      g2o_oplus(w.x[f], lay.rhs + cf, &w.n_oplus[f], S->ortho_after, &nx);
       if (ok) w.ev[f] = nx;
     }
     __syncthreads();
@@ -396,12 +372,10 @@ __global__ void __launch_bounds__(STEP_THREADS) g2o_step_kernel(G2oWork w) {
   }
   if (s_tobuild && !S->done) for (int f = tid; f < M; f += T) w.ev[f] = w.x[f];
   if (S->done)   // write the vertices of the problem back; every other frame keeps its pose bit for bit
-    for (int f = tid; f < M; f += T) if (w.col[f] >= 0) Rt_to_pose16(&w.x[f], w.poses16 + 16 * f);
+    for (int f = tid; f < M; f += T) if (lay.col[f] >= 0) Rt_to_pose16(&w.x[f], lay.poses16 + 16 * f);
   __syncthreads();
-  for (int i = tid; i < (int)(sizeof(G2oState) / sizeof(int32_t)); i += T)
-    reinterpret_cast<int32_t*>(w.S)[i] = reinterpret_cast<const int32_t*>(&s_state)[i];
-  __syncthreads();
-  if (tid == 0) { __threadfence(); w.host_flag[w.seq & 7] = (w.seq << 1) | (S->done ? 1 : 0); __threadfence_system(); }
+  copy_state(w.S, &s_state);
+  if (tid == 0) publish_step(lay, S->done);
 }
 
 }  // namespace mv

@@ -26,12 +26,26 @@ struct LmState {
   double radius, decrease_factor, x_cost, cand_cost, x_norm, initial_cost, model_cost_change, step_norm, gmax;
 };
 
+// The normal equations as both step kernels (lm_step_kernel, g2o_step_kernel) lay them out, gather them and report to the
+// host.  Built on the host from the free frames' local columns (mvicp.cu, build_normal_layout).
+struct NormalLayout {
+  const int32_t* col;        // [M] first local column or -1
+  // block-sparse gather lists (host-built, deterministic order)
+  const int32_t* hb_ptr; const int32_t* hb_row; const int32_t* hb_col; const int32_t* hc_edge; const int32_t* hc_sub; int32_t n_hblocks;
+  const int32_t* gb_ptr; const int32_t* gc_edge; const int32_t* gc_side;   // per frame
+  const int32_t* rlast; const int32_t* rfirst;   // envelope of the normal matrix: last row touching column j / first column of row r
+  const int32_t* rowbase;                        // skyline storage of the factor: entry (r, c) at Lg[rowbase[r] + c]; [n] = rhs row
+  double *Lg, *rhs;
+  int32_t l_in_smem;
+  double* poses16;
+  volatile int32_t* host_flag; // mapped pinned ring: (sequence << 1) | done, written at the end of every step
+  int32_t seq;
+};
+
 struct LmWork {
   LmState* S;
   const EdgeDev* edges;
   const double* eout;        // [E][EOUT]: pair matrix (144), pair gradient (12), cost at the evaluation point (summed over ranks)
-  volatile int32_t* host_flag; // mapped pinned ring: (sequence << 1) | done, written at the end of every step
-  int32_t seq;
   volatile int* peer_flags;    // this rank's flag array (written by the peers' edge kernels), null when not sharded over peer memory
   int32_t world, xseq;
   double* x;                 // [M][7] accepted point (all frames)
@@ -39,15 +53,8 @@ struct LmWork {
   Rt* Rt_eval;               // [M]
   double* K_eval;            // [M][36]
   FrameGen* G_eval;          // [M] general frame model (null unless a quaternion is not unit)
-  const int32_t* col;        // [M] first local column or -1
-  // block-sparse gather lists (host-built, deterministic order)
-  const int32_t* hb_ptr; const int32_t* hb_row; const int32_t* hb_col; const int32_t* hc_edge; const int32_t* hc_sub; int32_t n_hblocks;
-  const int32_t* gb_ptr; const int32_t* gc_edge; const int32_t* gc_side;   // per frame
-  const int32_t* rlast; const int32_t* rfirst;   // envelope of the normal matrix: last row touching column j / first column of row r
-  const int32_t* rowbase;                        // skyline storage of the factor: entry (r, c) at Lg[rowbase[r] + c]; [n] = rhs row
-  double *H, *g, *Hc, *gc, *scale, *diag, *Lg, *rhs, *step;
-  double* poses16;
-  int32_t l_in_smem;
+  NormalLayout lay;
+  double *H, *g, *Hc, *gc, *scale, *diag, *step;
   long long* prof;           // development aid (MVICP_STEP_PROFILE=1): clock64() stamps of the last solving launch, else null
 };
 
@@ -74,13 +81,57 @@ __device__ __forceinline__ double block_max(double v, double* red) {
   return red[32];
 }
 
+// ---- the normal-equation layout, shared by lm_step_kernel and g2o_step_kernel ------------------------------------
+// Dense normal matrix from the per-edge pair matrices: each listed 6x6 block summed over its (edge, sub-block) list in list
+// order.  Entries outside the listed blocks are zeroed once by the host when the layout is built and never written.
+__device__ __forceinline__ void gather_blocks(const NormalLayout& l, const double* eout, int n, double* H) {
+  for (int idx = threadIdx.x; idx < l.n_hblocks * 36; idx += blockDim.x) {
+    const int b = idx / 36, r = idx - 36 * b, i = r / 6, j = r - 6 * i;
+    double s = 0;
+    for (int c = l.hb_ptr[b]; c < l.hb_ptr[b + 1]; ++c) {
+      const int e = l.hc_edge[c], sub = l.hc_sub[c];   // sub: 0 ss, 1 sk, 2 ks, 3 kk
+      s += eout[(size_t)EOUT * e + (6 * (sub >> 1) + i) * 12 + 6 * (sub & 1) + j];
+    }
+    H[(size_t)(l.hb_row[b] + i) * n + l.hb_col[b] + j] = s;
+  }
+}
+// Gradient of every frame with a column: its (edge, side) pair gradients summed in list order
+__device__ __forceinline__ void gather_gradient(const NormalLayout& l, const double* eout, int M, double* g) {
+  for (int idx = threadIdx.x; idx < M * 6; idx += blockDim.x) {
+    const int f = idx / 6, i = idx - 6 * f;
+    if (l.col[f] < 0) continue;
+    double s = 0;
+    for (int c = l.gb_ptr[f]; c < l.gb_ptr[f + 1]; ++c) s += eout[(size_t)EOUT * l.gc_edge[c] + 144 + 6 * l.gc_side[c] + i];
+    g[l.col[f] + i] = s;
+  }
+}
+// Total cost: edges summed in a fixed order (thread t takes edges t, t + T, ...; then the block tree) -- the same on every rank
+__device__ __forceinline__ double edge_cost_sum(const double* eout, int E, double* red) {
+  double s = 0.0;
+  for (int e = threadIdx.x; e < E; e += blockDim.x) s += eout[(size_t)EOUT * e + 156];
+  return block_sum(s, red);
+}
+// A step kernel works on a shared-memory copy of its state (dozens of dependent scalar reads per step) and writes it back once
+// at the end; nobody else touches the state while the kernel runs
+template <typename State> __device__ __forceinline__ void copy_state(State* dst, const State* src) {
+  for (int i = threadIdx.x; i < (int)(sizeof(State) / sizeof(int32_t)); i += blockDim.x)
+    reinterpret_cast<int32_t*>(dst)[i] = reinterpret_cast<const int32_t*>(src)[i];
+  __syncthreads();
+}
+// One thread tells the host that this step ran: (sequence << 1) | done into the mapped ring, after every write of the step
+__device__ __forceinline__ void publish_step(const NormalLayout& l, bool done) {
+  __threadfence();
+  l.host_flag[l.seq & 7] = (l.seq << 1) | (done ? 1 : 0);
+  __threadfence_system();
+}
+
 // Per-frame set-up before the first evaluation: poses -> parameters, functor rotation, tangent map.
 __global__ void lm_init_kernel(LmWork w) {
   LmState* S = w.S;
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= S->M) return;
   double x[7] = {0, 0, 0, 0, 0, 0, 0};
-  param_of_pose(S->param, w.poses16 + 16 * f, x);
+  param_of_pose(S->param, w.lay.poses16 + 16 * f, x);
   if (S->param != PARAM_AA) {
     const double n2 = x[0] * x[0] + x[1] * x[1] + x[2] * x[2] + x[3] * x[3];
     if (!(fabs(n2 - 1.0) <= 1e-9)) atomicExch(&S->nonrigid, 1);
@@ -260,17 +311,14 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
   extern __shared__ double smem[];
   __shared__ double red[40];
   __shared__ int s_flag;
-  if (w.S->done) { if (threadIdx.x == 0) { w.host_flag[w.seq & 7] = (w.seq << 1) | 1; __threadfence_system(); } return; }
+  if (w.S->done) { if (threadIdx.x == 0) publish_step(w.lay, true); return; }
   const int tid = threadIdx.x, T = blockDim.x;
-  // the state machine works on a shared-memory copy of LmState (dozens of dependent scalar reads per step) and writes it
-  // back once at the end; nobody else touches it while this kernel runs
   __shared__ LmState s_state;
-  for (int i = tid; i < (int)(sizeof(LmState) / sizeof(int32_t)); i += T)
-    reinterpret_cast<int32_t*>(&s_state)[i] = reinterpret_cast<const int32_t*>(w.S)[i];
-  __syncthreads();
+  copy_state(&s_state, w.S);
   LmState* S = &s_state;
   const int n = S->n, M = S->M, E = S->E, param = S->param;
-  long long* prof = w.prof ? w.prof + 16 * (w.seq & 3) : nullptr;   // one row of stamps per launch, the last four launches kept
+  const NormalLayout& lay = w.lay;
+  long long* prof = w.prof ? w.prof + 16 * (lay.seq & 3) : nullptr;   // one row of stamps per launch, the last four launches kept
 #define MV_STAMP(i) do { if (prof && tid == 0) prof[i] = clock64(); } while (0)
   MV_STAMP(0);
   if (w.peer_flags) {   // wait until every rank's edge kernel has delivered this iteration's pair matrices
@@ -284,31 +332,13 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
   }
   // dynamic shared memory: [scratch 2(n+1) | dg (n+1) | L (skyline) when it fits]
   double* colj = smem; double* dg = smem + 2 * (S->n + 1);
-  double* L = w.l_in_smem ? smem + 3 * (S->n + 1) : w.Lg;
+  double* L = lay.l_in_smem ? smem + 3 * (S->n + 1) : lay.Lg;
 
   // ================= 1. gather the per-edge pair matrices (lm_edge_kernel) into Hc, gc; total cost ===================
-  // (entries outside the listed blocks are zeroed once by the host when the block structure is built and never written)
-  for (int idx = tid; idx < w.n_hblocks * 36; idx += T) {   // gather into the dense matrix, fixed order
-    const int b = idx / 36, r = idx - 36 * b, i = r / 6, j = r - 6 * i;
-    double s = 0;
-    for (int c = w.hb_ptr[b]; c < w.hb_ptr[b + 1]; ++c) {
-      const int e = w.hc_edge[c], sub = w.hc_sub[c];   // sub: 0 ss, 1 sk, 2 ks, 3 kk
-      s += w.eout[(size_t)EOUT * e + (6 * (sub >> 1) + i) * 12 + 6 * (sub & 1) + j];
-    }
-    w.Hc[(size_t)(w.hb_row[b] + i) * n + w.hb_col[b] + j] = s;
-  }
-  for (int idx = tid; idx < M * 6; idx += T) {
-    const int f = idx / 6, i = idx - 6 * f;
-    if (w.col[f] < 0) continue;
-    double s = 0;
-    for (int c = w.gb_ptr[f]; c < w.gb_ptr[f + 1]; ++c) s += w.eout[(size_t)EOUT * w.gc_edge[c] + 144 + 6 * w.gc_side[c] + i];
-    w.gc[w.col[f] + i] = s;
-  }
+  gather_blocks(lay, w.eout, n, w.Hc);
+  gather_gradient(lay, w.eout, M, w.gc);
   __syncthreads();
-  // total cost: edges summed in a fixed order (thread t takes edges t, t + T, ...; then the block tree) -- the same on every rank
-  double eval_cost = 0.0;
-  for (int e = tid; e < E; e += T) eval_cost += w.eout[(size_t)EOUT * e + 156];
-  eval_cost = block_sum(eval_cost, red);
+  const double eval_cost = edge_cost_sum(w.eout, E, red);
 
   MV_STAMP(1);
   // ================= 2. accept / reject / terminate =================================================
@@ -348,9 +378,9 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
   __syncthreads();
   take = s_flag != 0;
   if (take) {
-    for (int idx = tid; idx < w.n_hblocks * 36; idx += T) {
+    for (int idx = tid; idx < lay.n_hblocks * 36; idx += T) {
       const int b = idx / 36, r = idx - 36 * b, i = r / 6, j = r - 6 * i;
-      const size_t at = (size_t)(w.hb_row[b] + i) * n + w.hb_col[b] + j;
+      const size_t at = (size_t)(lay.hb_row[b] + i) * n + lay.hb_col[b] + j;
       w.H[at] = w.Hc[at];
     }
     for (int idx = tid; idx < n; idx += T) w.g[idx] = w.gc[idx];
@@ -361,11 +391,11 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
     // x_norm over the free blocks, and the gradient test |x - Plus(x, -g)|_inf
     double xs = 0.0, gm = 0.0;
     for (int f = tid; f < M; f += T) {
-      if (w.col[f] < 0) continue;
+      if (lay.col[f] < 0) continue;
       const int G = S->G;
       double xf[7], ng[6], xp[7];
       for (int i = 0; i < G; ++i) { xf[i] = w.x[7 * f + i]; xs += xf[i] * xf[i]; }
-      for (int i = 0; i < 6; ++i) ng[i] = -w.g[w.col[f] + i];
+      for (int i = 0; i < 6; ++i) ng[i] = -w.g[lay.col[f] + i];
       param_plus(param, xf, ng, xp);
       for (int i = 0; i < G; ++i) gm = fmax(gm, fabs(xf[i] - xp[i]));
     }
@@ -400,31 +430,31 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
     __syncthreads();
     for (int i = tid >> 5; i < n; i += T >> 5) {          // one warp per row, only the row's profile (see chol_solve)
       const double si = w.scale[i];
-      const int rbi = w.rowbase[i];
-      for (int j = w.rfirst[i] + (tid & 31); j <= i; j += 32) {
+      const int rbi = lay.rowbase[i];
+      for (int j = lay.rfirst[i] + (tid & 31); j <= i; j += 32) {
         double v = si * w.H[(size_t)i * n + j] * w.scale[j];
         if (i == j) { const double ldg = sqrt(w.diag[i] / radius); v += ldg * ldg; }
         L[rbi + j] = v;
       }
     }
-    { const int rbn = w.rowbase[n]; for (int j = tid; j < n; j += T) L[rbn + j] = w.scale[j] * w.g[j]; }
+    { const int rbn = lay.rowbase[n]; for (int j = tid; j < n; j += T) L[rbn + j] = w.scale[j] * w.g[j]; }
     __syncthreads();
     MV_STAMP(3);
-    bool ok = chol_solve(L, w.rowbase, n, colj, dg, w.rhs, w.rlast, w.rfirst, prof);
+    bool ok = chol_solve(L, lay.rowbase, n, colj, dg, lay.rhs, lay.rlast, lay.rfirst, prof);
     MV_STAMP(4);
     double bad = 0.0;
-    if (ok) for (int j = tid; j < n; j += T) if (!isfinite(w.rhs[j])) bad = 1.0;
+    if (ok) for (int j = tid; j < n; j += T) if (!isfinite(lay.rhs[j])) bad = 1.0;
     bad = block_sum(bad, red);
     ok = ok && (bad == 0.0);
     double mcc = 0.0;
     if (ok) {
-      for (int j = tid; j < n; j += T) w.step[j] = -w.rhs[j];
+      for (int j = tid; j < n; j += T) w.step[j] = -lay.rhs[j];
       __syncthreads();
       // model_cost_change = -(J s).(r + J s / 2) = -s.g~ - 1/2 s^T H~ s; with (H~ + D^2) y = g~ and s = -y this is
       // 1/2 (y.g~ + sum D_i^2 y_i^2): O(n) instead of O(n^2)
       double acc = 0.0;
       for (int i = tid; i < n; i += T) {
-        const double y = w.rhs[i];
+        const double y = lay.rhs[i];
         acc += 0.5 * (y * w.scale[i] * w.g[i] + (w.diag[i] / radius) * y * y);
       }
       mcc = block_sum(acc, red);
@@ -447,8 +477,8 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
       const int G = S->G;
       double xf[7], d[6], xp[7] = {0, 0, 0, 0, 0, 0, 0};
       for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * f + i];
-      if (w.col[f] >= 0) {
-        for (int i = 0; i < 6; ++i) d[i] = w.step[w.col[f] + i] * w.scale[w.col[f] + i];
+      if (lay.col[f] >= 0) {
+        for (int i = 0; i < 6; ++i) d[i] = w.step[lay.col[f] + i] * w.scale[lay.col[f] + i];
         param_plus(param, xf, d, xp);
         for (int i = 0; i < G; ++i) sn += (xf[i] - xp[i]) * (xf[i] - xp[i]);
       } else for (int i = 0; i < 7; ++i) xp[i] = xf[i];
@@ -470,15 +500,13 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
   if (S->done) {
     for (int f = tid; f < M; f += T) {
       double xf[7]; for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * f + i];
-      pose_of_param(param, xf, w.poses16 + 16 * f);
+      pose_of_param(param, xf, lay.poses16 + 16 * f);
     }
   }
   __syncthreads();
-  for (int i = tid; i < (int)(sizeof(LmState) / sizeof(int32_t)); i += T)
-    reinterpret_cast<int32_t*>(w.S)[i] = reinterpret_cast<const int32_t*>(&s_state)[i];
-  __syncthreads();
+  copy_state(w.S, &s_state);
   MV_STAMP(6);
-  if (tid == 0) { __threadfence(); w.host_flag[w.seq & 7] = (w.seq << 1) | (S->done ? 1 : 0); __threadfence_system(); }
+  if (tid == 0) publish_step(lay, S->done);
   MV_STAMP(7);
 #undef MV_STAMP
 }

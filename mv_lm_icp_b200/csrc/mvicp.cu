@@ -56,8 +56,13 @@ static int fail(int code, const char* fmt, ...) {
   } while (0)
 #define RET(call) do { int r__ = (call); if (r__ != MVICP_OK) return r__; } while (0)
 
+// A device allocation that only grows; freed with its owner (the context's device must be current then, as in mvicp_destroy)
 struct DevBuf {
   void* p = nullptr; size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { release(); }
   int reserve(size_t bytes) {
     if (bytes <= cap) return MVICP_OK;
     if (p) cudaFree(p);
@@ -117,7 +122,8 @@ struct mvicp_ctx {
   DevBuf d_state, d_x, d_cand, d_Rt, d_K, d_col, d_H, d_g, d_Hc, d_gc, d_scale, d_diag, d_L, d_rhs, d_step,
       d_eout, d_hb_ptr, d_hb_row, d_hb_col, d_hc_edge, d_hc_sub, d_gb_ptr, d_gc_edge, d_gc_side, d_posegather, d_rlast, d_rfirst, d_rowbase, d_gen;
   int64_t l_size = 0;          // doubles of the factor's skyline storage (row profiles + rhs row)
-  int n_free = 0, n_hblocks = 0;
+  int n_free = 0;
+  NormalLayout lay{};          // device view of the layout last built (build_normal_layout), poses16 set by each solve
   std::vector<int32_t> h_col;
   void* h_state = nullptr;     // pinned staging of LmState
   volatile int32_t* h_flag = nullptr; volatile int32_t* d_flag = nullptr;   // mapped pinned ring written by lm_step_kernel
@@ -398,23 +404,13 @@ void mvicp_destroy(mvicp_ctx* c) {
   if (c->xbuf) cudaFree(c->xbuf);
   if (c->comm) ncclCommDestroy(c->comm);
   for (void* p : c->frame_allocs) cudaFree(p);
-  DevBuf* bufs[] = {&c->d_frames, &c->d_poses, &c->d_edges, &c->d_xf, &c->d_corr, &c->d_d2, &c->d_count, &c->d_sel, &c->d_hist,
-                    &c->d_weight, &c->d_median, &c->d_selcand, &c->d_selcand_n, &c->d_sel_cnt, &c->d_sel_win, &c->d_certs, &c->d_cert_cnt, &c->d_todo, &c->d_todo_n, &c->d_knn_tiles, &c->d_eval_tiles, &c->d_edge_tile_begin, &c->d_partial,
-                    &c->d_state, &c->d_x, &c->d_cand, &c->d_Rt, &c->d_K, &c->d_col, &c->d_H, &c->d_g, &c->d_Hc,
-                    &c->d_gc, &c->d_scale, &c->d_diag, &c->d_L, &c->d_rhs, &c->d_step, &c->d_eout,
-                    &c->d_hb_ptr, &c->d_hb_row, &c->d_hb_col, &c->d_hc_edge, &c->d_hc_sub, &c->d_gb_ptr, &c->d_gc_edge,
-                    &c->d_gc_side, &c->d_posegather, &c->d_rlast, &c->d_rfirst, &c->d_rowbase, &c->d_gen, &c->d_obb, &c->d_single, &c->d_prof, &c->d_tile_count, &c->d_tile_off, &c->d_edge_off, &c->d_recs,
-                    &c->d_cpq, &c->d_cpr, &c->d_set_win, &c->d_set_bad, &c->d_knn_nor,
-                    &c->d_g2o_state, &c->d_g2o_x, &c->d_g2o_ev, &c->d_g2o_nop, &c->d_g2o_chi, &c->d_g2o_trace, &c->d_g2o_tiles,
-                    &c->d_g2o_tile_begin, &c->d_g2o_cnt};
-  for (DevBuf* b : bufs) b->release();
   for (auto& ev : c->ev) if (ev) cudaEventDestroy(ev);
   for (auto& ev : c->eval_ev) cudaEventDestroy(ev);
   if (c->h_state) cudaFreeHost(c->h_state);
   if (c->h_flag) cudaFreeHost((void*)c->h_flag);
 
   if (c->own_stream && c->stream) cudaStreamDestroy(c->stream);
-  delete c;
+  delete c;   // frees every DevBuf, on the device set above
 }
 
 }  // extern "C"
@@ -1059,26 +1055,22 @@ int mvicp_closest_points_device(mvicp_ctx* c, int32_t frame, const double* q, in
   return launch_closest_points(c, frame, q, n, reinterpret_cast<long long*>(idx), d2);
 }
 
-// ---- LM ------------------------------------------------------------------------------------------
-static int prepare_lm(mvicp_ctx* c, int n) {
+// ---- the normal-equation layout and the host loop shared by both solvers (lm_step.cuh NormalLayout) -----------------
+// Block structure of the normal matrix over the local columns c->h_col (n of them): edge e, when active[e], puts its pair
+// matrix's ss / sk / ks / kk sub-blocks into blocks (s, s) / (s, k) / (k, s) / (k, k) and its (e, side) pair gradient into frame
+// s's / k's gradient, wherever those ends have a column.  Uploads the gather lists, the envelope and the skyline layout of the
+// factor, and zeroes the dense normal matrix.
+static int build_normal_layout(mvicp_ctx* c, int n, const std::vector<uint8_t>& active) {
   const int M = c->M, E = c->E;
-  RET(c->d_state.reserve(sizeof(LmState)));
-  RET(c->d_x.reserve(sizeof(double) * 7 * M)); RET(c->d_cand.reserve(sizeof(double) * 7 * M));
-  RET(c->d_Rt.reserve(sizeof(Rt) * M)); RET(c->d_K.reserve(sizeof(double) * 36 * M));
-  RET(c->d_col.reserve(sizeof(int32_t) * M));
-  RET(c->d_H.reserve(sizeof(double) * n * n)); RET(c->d_Hc.reserve(sizeof(double) * n * n));
-  RET(c->d_g.reserve(sizeof(double) * n)); RET(c->d_gc.reserve(sizeof(double) * n)); RET(c->d_scale.reserve(sizeof(double) * n));
-  RET(c->d_diag.reserve(sizeof(double) * n)); RET(c->d_rhs.reserve(sizeof(double) * n)); RET(c->d_step.reserve(sizeof(double) * n));
-  RET(c->d_eout.reserve(sizeof(double) * EOUT * E));
-  return MVICP_OK;
-}
-
-// Block structure of the normal matrix over n local columns (c->h_col): blk[r * M + q] lists the (edge, sub-block) pairs that
-// sum into block (r, q) (sub 0 ss, 1 sk, 2 ks, 3 kk of the edge's pair matrix), gl[f] the (edge, side) pairs of frame f's
-// gradient.  Uploads the gather lists, the envelope and the skyline layout of the factor, and zeroes the dense matrices.
-typedef std::vector<std::vector<std::pair<int, int>>> BlockLists;
-static int upload_lm_structure(mvicp_ctx* c, int n, const BlockLists& blk, const BlockLists& gl) {
-  const int M = c->M;
+  std::vector<std::vector<std::pair<int, int>>> blk((size_t)M * M), gl(M);
+  for (int e = 0; e < E; ++e) {
+    if (!active[e]) continue;
+    const int s = c->h_edges[e].src, k = c->h_edges[e].dst;
+    const bool fs = c->h_col[s] >= 0, fk = c->h_col[k] >= 0;
+    if (fs) { blk[(size_t)s * M + s].push_back({e, 0}); gl[s].push_back({e, 0}); }
+    if (fs && fk) { blk[(size_t)s * M + k].push_back({e, 1}); blk[(size_t)k * M + s].push_back({e, 2}); }
+    if (fk) { blk[(size_t)k * M + k].push_back({e, 3}); gl[k].push_back({e, 1}); }
+  }
   std::vector<int32_t> hb_ptr{0}, hb_row, hb_col, hc_edge, hc_sub, gb_ptr{0}, gc_edge, gc_side;
   for (int r = 0; r < M; ++r)
     for (int q = 0; q < M; ++q) {
@@ -1089,11 +1081,11 @@ static int upload_lm_structure(mvicp_ctx* c, int n, const BlockLists& blk, const
       hb_ptr.push_back((int32_t)hc_edge.size());
     }
   for (int f = 0; f < M; ++f) { for (auto& pr : gl[f]) { gc_edge.push_back(pr.first); gc_side.push_back(pr.second); } gb_ptr.push_back((int32_t)gc_edge.size()); }
-  c->n_hblocks = (int)hb_row.size();
+  const int n_hblocks = (int)hb_row.size();
   // envelope: first structurally non-zero column of every row, and the last row that reaches column j
   std::vector<int32_t> rfirst(n), rlast(n);
   for (int r = 0; r < n; ++r) rfirst[r] = (r / 6) * 6;
-  for (int b = 0; b < c->n_hblocks; ++b)
+  for (int b = 0; b < n_hblocks; ++b)
     if (hb_col[b] < hb_row[b]) for (int i = 0; i < 6; ++i) rfirst[hb_row[b] + i] = std::min(rfirst[hb_row[b] + i], hb_col[b]);
   for (int j = 0; j < n; ++j) { rlast[j] = j; }
   for (int r = 0; r < n; ++r) for (int j = rfirst[r]; j <= r; ++j) rlast[j] = std::max(rlast[j], r);
@@ -1115,14 +1107,20 @@ static int upload_lm_structure(mvicp_ctx* c, int n, const BlockLists& blk, const
   c->l_size = at;
   RET(c->d_L.reserve(sizeof(double) * (size_t)at));
   RET(up(c->d_rowbase, rowbase));
-  // the step kernel writes only the listed blocks of the dense normal matrix; everything else stays zero from here
+  RET(c->d_H.reserve(sizeof(double) * n * n)); RET(c->d_g.reserve(sizeof(double) * n)); RET(c->d_rhs.reserve(sizeof(double) * n));
+  RET(c->d_eout.reserve(sizeof(double) * EOUT * E));
+  // the step kernels write only the listed blocks of the dense normal matrix; everything else stays zero from here
   CU(cudaMemsetAsync(c->d_H.p, 0, sizeof(double) * (size_t)n * n, c->stream));
-  CU(cudaMemsetAsync(c->d_Hc.p, 0, sizeof(double) * (size_t)n * n, c->stream));
-
   CU(cudaStreamSynchronize(c->stream));   // the host vectors above must outlive their copies
+  NormalLayout& l = c->lay;   // (the ring sequence and l_in_smem are set by run_steps)
+  l.col = c->d_col.as<int32_t>();
+  l.hb_ptr = c->d_hb_ptr.as<int32_t>(); l.hb_row = c->d_hb_row.as<int32_t>(); l.hb_col = c->d_hb_col.as<int32_t>();
+  l.hc_edge = c->d_hc_edge.as<int32_t>(); l.hc_sub = c->d_hc_sub.as<int32_t>(); l.n_hblocks = n_hblocks;
+  l.gb_ptr = c->d_gb_ptr.as<int32_t>(); l.gc_edge = c->d_gc_edge.as<int32_t>(); l.gc_side = c->d_gc_side.as<int32_t>();
+  l.rlast = c->d_rlast.as<int32_t>(); l.rfirst = c->d_rfirst.as<int32_t>(); l.rowbase = c->d_rowbase.as<int32_t>();
+  l.Lg = c->d_L.as<double>(); l.rhs = c->d_rhs.as<double>(); l.host_flag = c->d_flag;
   return MVICP_OK;
 }
-
 }  // extern "C"
 template <bool F32> static void launch_eval(mvicp_ctx* c, int cost, int robust, const int* done_flag) {
   const int nt = c->n_eval_tiles;
@@ -1151,6 +1149,100 @@ template <bool F32> static void launch_eval_general(mvicp_ctx* c, int param, int
   if (cost == COST_P2P) { MV_EVALG(COST_P2P); } else if (cost == COST_P2PLANE) { MV_EVALG(COST_P2PLANE); } else { MV_EVALG(COST_MIXED); }
 #undef MV_EVALG
 }
+
+// The pipelined loop of both solvers: evaluation i+1 is enqueued before the host learns whether step i finished the solve,
+// so the GPU never waits for the host; kernels issued after termination exit at once.  `eval()` enqueues the streaming
+// evaluation (timed by a pair of events), `step(dyn)` the rest of the iteration, ending with the step kernel `kernel`, which
+// publishes (lay.seq << 1) | done into the mapped ring.
+template <typename Kernel, typename Eval, typename Step>
+static int run_steps(mvicp_ctx* c, Kernel kernel, int n, int64_t max_evals, const char* what, NormalLayout& lay, Eval&& eval, Step&& step) {
+  const size_t l_bytes = sizeof(double) * (size_t)c->l_size;
+  const size_t vec_bytes = sizeof(double) * 3 * (size_t)(n + 1);
+  lay.l_in_smem = (l_bytes + vec_bytes) <= 220 * 1024 ? 1 : 0;
+  const size_t dyn = vec_bytes + (lay.l_in_smem ? l_bytes : 0);
+  CU(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  for (int i = 0; i < 8; ++i) c->h_flag[i] = 0;
+  c->eval_ev_used = 0;
+  int64_t issued = 0, seen = 0;
+  auto issue = [&]() -> int {
+    if ((int)c->eval_ev.size() < c->eval_ev_used + 2) { cudaEvent_t a, b; CU(cudaEventCreate(&a)); CU(cudaEventCreate(&b)); c->eval_ev.push_back(a); c->eval_ev.push_back(b); }
+    CU(cudaEventRecord(c->eval_ev[c->eval_ev_used], c->stream));
+    eval();
+    CU(cudaEventRecord(c->eval_ev[c->eval_ev_used + 1], c->stream));
+    c->eval_ev_used += 2;
+    lay.seq = (int32_t)(issued + 1);
+    RET(step(dyn));
+    ++issued;
+    return MVICP_OK;
+  };
+  RET(issue());
+  while (true) {
+    if (issued - seen < 2 && issued <= max_evals) RET(issue());
+    // the step kernel publishes (sequence << 1 | done) into mapped pinned memory: spin on it, no stream round trip
+    const int32_t want = (int32_t)(seen + 1);
+    int32_t v;
+    long spins = 0;
+    while (((v = c->h_flag[want & 7]) >> 1) != want) {
+      if ((++spins & 0xfffff) == 0 && cudaStreamQuery(c->stream) != cudaErrorNotReady) {   // kernels died or stream drained
+        v = c->h_flag[want & 7];
+        if ((v >> 1) != want) { CU(cudaGetLastError()); return fail(MVICP_ERR_CUDA, "%s step %d never reported", what, want); }
+        break;
+      }
+    }
+    ++seen;
+    if ((v & 1) != 0 || seen > max_evals) break;
+  }
+  return MVICP_OK;
+}
+
+// End of a solve: the solver state and every pose back to the host.  The host pose mirror follows the device:
+// mvicp_pose_graph_knn and mvicp_set_poses' "same poses as last handed out" test read it.
+static int read_back_solve(mvicp_ctx* c, void* state, const void* d_state, size_t bytes) {
+  CU(cudaEventRecord(c->ev[4], c->stream));
+  CU(cudaMemcpyAsync(state, d_state, bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaMemcpyAsync(c->h_poses.data(), c->d_poses.p, sizeof(double) * 16 * c->M, cudaMemcpyDeviceToHost, c->stream));
+  CU(cudaStreamSynchronize(c->stream));
+  CU(cudaGetLastError());
+  c->ev_lm = true;
+  return MVICP_OK;
+}
+
+// Edge ownership follows the fixed flags (a fixed src frame's edges belong to nobody): refresh the layout when a solve has
+// just fixed frame 0 (frames[0]->fixed = true, icp-ceres.cpp:242-244, icp-g2o.cpp:182-186) or mvicp_set_poses changed them.
+static int refresh_if_fixed_changed(mvicp_ctx* c) {
+  bool stale = false;
+  for (int e = 0; e < c->E; ++e) if ((c->edge_owner[e] < 0) != (c->fixed[c->h_edges[e].src] != 0)) stale = true;
+  if (!stale) return MVICP_OK;
+  if (c->world > 1) return fail(MVICP_ERR_STATE, "sharded run: frame 0 was free when the edges were distributed; fix it (mvicp_set_poses) before mvicp_correspond");
+  return refresh_after_fixed_change(c);
+}
+
+// The two-frame problem of mvicp_pairwise*: frame 0 = dst (fixed at the identity), frame 1 = src (from the identity), edge
+// 1 -> 0 with identity matches.  Runs `solve(c)` on it, copies pose 1 out and destroys the context, keeping the error text.
+template <typename Solve>
+static int run_pairwise(const mvicp_config* cfg, const double* src, const double* dst, const double* nor, int64_t n, double* pose16_out,
+                        Solve&& solve) {
+  mvicp_ctx* c = nullptr;
+  RET(mvicp_create(cfg, &c));
+  const double* pts[2] = {dst, src}; const double* nrs[2] = {nor, nor};   // src normals are never read
+  const int64_t np[2] = {n, n};
+  int rc = mvicp_set_frames(c, 2, pts, nor ? nrs : nullptr, np);
+  const int32_t es = 1, ed = 0;
+  if (rc == MVICP_OK) rc = mvicp_set_graph(c, 1, &es, &ed);
+  if (rc == MVICP_OK) {
+    std::vector<int32_t> id(n); std::iota(id.begin(), id.end(), 0);
+    rc = mvicp_set_edge(c, 0, id.data(), id.data(), n, 1.0f);
+  }
+  if (rc == MVICP_OK) rc = solve(c);
+  std::vector<double> poses(32);
+  if (rc == MVICP_OK) rc = mvicp_get_poses(c, poses.data());
+  if (rc == MVICP_OK) std::memcpy(pose16_out, poses.data() + 16, sizeof(double) * 16);
+  const std::string keep = g_err;
+  mvicp_destroy(c);
+  g_err = keep;
+  return rc;
+}
+
 extern "C" {
 int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt_in, mvicp_lm_summary* summary) {
   if (!c || !c->M || !c->E) return fail(MVICP_ERR_STATE, "mvicp_optimize: frames and graph must be set first");
@@ -1168,32 +1260,19 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
     if (summary) { std::memset(summary, 0, sizeof *summary); summary->termination = MVICP_TERM_GRADIENT_TOLERANCE; }
     return MVICP_OK;
   }
-  // ownership may depend on `fixed`: refresh the edge table if it changed
-  bool stale = false;
-  for (int e = 0; e < E; ++e) {
-    if ((c->edge_owner[e] < 0) != (c->fixed[c->h_edges[e].src] != 0)) stale = true;
-  }
-  if (stale) {
-    if (c->world > 1) return fail(MVICP_ERR_STATE, "sharded run: frame 0 was free when the edges were distributed; fix it (mvicp_set_poses) before mvicp_correspond");
-    RET(refresh_after_fixed_change(c));
-  }
-  // the gather lists / envelope depend only on the graph and the fixed flags: build and upload them when those change
+  RET(refresh_if_fixed_changed(c));
+  // the layout depends only on the graph and the fixed flags: build and upload it when those change
   std::vector<uint8_t> key(c->fixed); key.push_back((uint8_t)(c->graph_gen & 0xff)); key.push_back((uint8_t)((c->graph_gen >> 8) & 0xff));
   if (key != c->lm_key) {
-  RET(prepare_lm(c, n));
-    // block-sparse gather lists
-    std::vector<std::vector<std::pair<int, int>>> blk((size_t)M * M);
-    std::vector<std::vector<std::pair<int, int>>> gl(M);
-    for (int e = 0; e < E; ++e) {
-      const int s = c->h_edges[e].src, k = c->h_edges[e].dst;
-      if (c->fixed[s]) continue;
-      blk[(size_t)s * M + s].push_back({e, 0}); gl[s].push_back({e, 0});
-      if (!c->fixed[k]) {
-        blk[(size_t)s * M + k].push_back({e, 1}); blk[(size_t)k * M + s].push_back({e, 2}); blk[(size_t)k * M + k].push_back({e, 3});
-        gl[k].push_back({e, 1});
-      }
-    }
-    RET(upload_lm_structure(c, n, blk, gl));
+    RET(c->d_state.reserve(sizeof(LmState)));
+    RET(c->d_x.reserve(sizeof(double) * 7 * M)); RET(c->d_cand.reserve(sizeof(double) * 7 * M));
+    RET(c->d_Rt.reserve(sizeof(Rt) * M)); RET(c->d_K.reserve(sizeof(double) * 36 * M));
+    RET(c->d_Hc.reserve(sizeof(double) * n * n)); RET(c->d_gc.reserve(sizeof(double) * n)); RET(c->d_scale.reserve(sizeof(double) * n));
+    RET(c->d_diag.reserve(sizeof(double) * n)); RET(c->d_step.reserve(sizeof(double) * n));
+    CU(cudaMemsetAsync(c->d_Hc.p, 0, sizeof(double) * (size_t)n * n, c->stream));
+    std::vector<uint8_t> active(E);
+    for (int e = 0; e < E; ++e) active[e] = !c->fixed[c->h_edges[e].src];
+    RET(build_normal_layout(c, n, active));
     c->lm_key = key;
   }
   LmState st; std::memset(&st, 0, sizeof st);
@@ -1204,45 +1283,27 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
 
   LmWork w{};
   w.S = c->d_state.as<LmState>(); w.edges = c->d_edges.as<EdgeDev>(); w.eout = c->d_eout.as<double>();
-  w.host_flag = c->d_flag;
   if (std::getenv("MVICP_STEP_PROFILE")) { RET(c->d_prof.reserve(sizeof(long long) * 64)); w.prof = c->d_prof.as<long long>(); }
   c->nonrigid = poses_nonrigid(c->h_poses.data(), M);   // the mirror follows every solve and every mvicp_set_poses
   const bool general = c->nonrigid && param != PARAM_AA;
   if (general) { RET(c->d_gen.reserve(sizeof(FrameGen) * M)); RET(c->d_partial.reserve(sizeof(double) * GBLK * std::max<size_t>(1, c->n_eval_tiles))); }
   w.G_eval = general ? c->d_gen.as<FrameGen>() : nullptr;
   w.x = c->d_x.as<double>(); w.cand = c->d_cand.as<double>(); w.Rt_eval = c->d_Rt.as<Rt>(); w.K_eval = c->d_K.as<double>();
-  w.col = c->d_col.as<int32_t>();
-  w.hb_ptr = c->d_hb_ptr.as<int32_t>(); w.hb_row = c->d_hb_row.as<int32_t>(); w.hb_col = c->d_hb_col.as<int32_t>();
-  w.hc_edge = c->d_hc_edge.as<int32_t>(); w.hc_sub = c->d_hc_sub.as<int32_t>(); w.n_hblocks = c->n_hblocks;
-  w.rlast = c->d_rlast.as<int32_t>(); w.rfirst = c->d_rfirst.as<int32_t>(); w.rowbase = c->d_rowbase.as<int32_t>();
-  w.gb_ptr = c->d_gb_ptr.as<int32_t>(); w.gc_edge = c->d_gc_edge.as<int32_t>(); w.gc_side = c->d_gc_side.as<int32_t>();
+  w.lay = c->lay; w.lay.poses16 = c->d_poses.as<double>();
   w.H = c->d_H.as<double>(); w.g = c->d_g.as<double>(); w.Hc = c->d_Hc.as<double>(); w.gc = c->d_gc.as<double>();
-  w.scale = c->d_scale.as<double>(); w.diag = c->d_diag.as<double>(); w.Lg = c->d_L.as<double>(); w.rhs = c->d_rhs.as<double>();
-  w.step = c->d_step.as<double>(); w.poses16 = c->d_poses.as<double>();
-  const size_t l_bytes = sizeof(double) * (size_t)c->l_size;
-  const size_t vec_bytes = sizeof(double) * 3 * (size_t)(n + 1);
-  w.l_in_smem = (l_bytes + vec_bytes) <= 220 * 1024 ? 1 : 0;
-  const size_t dyn = vec_bytes + (w.l_in_smem ? l_bytes : 0);
-  CU(cudaFuncSetAttribute(lm_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  w.scale = c->d_scale.as<double>(); w.diag = c->d_diag.as<double>(); w.step = c->d_step.as<double>();
 
   CU(cudaEventRecord(c->ev[3], c->stream));
   lm_init_kernel<<<(M + 63) / 64, 64, 0, c->stream>>>(w);
   c->stats.kernel_launches += 1;
-  // The loop is pipelined one iteration deep: iteration i+1 is enqueued before the host learns whether iteration i
-  // terminated, so the GPU never waits for the host; kernels of an iteration issued after termination exit at once.
   const int max_evals = opt.max_num_iterations + 2;
-  for (int i = 0; i < 8; ++i) c->h_flag[i] = 0;
-  c->eval_ev_used = 0;
   const bool use_p2p = c->comm && c->world > 1 && c->p2p_ok && E <= mvicp_ctx::X_ECAP;
-  int issued = 0, seen = 0;
   const int* done_flag = &w.S->done;
-  auto issue = [&]() -> int {
-    if ((int)c->eval_ev.size() < c->eval_ev_used + 2) { cudaEvent_t a, b; CU(cudaEventCreate(&a)); CU(cudaEventCreate(&b)); c->eval_ev.push_back(a); c->eval_ev.push_back(b); }
-    CU(cudaEventRecord(c->eval_ev[c->eval_ev_used], c->stream));
+  auto eval = [&]() {
     if (general) { if (c->f32) launch_eval_general<true>(c, param, cost, st.robust, done_flag); else launch_eval_general<false>(c, param, cost, st.robust, done_flag); }
     else if (c->f32) launch_eval<true>(c, cost, st.robust, done_flag); else launch_eval<false>(c, cost, st.robust, done_flag);
-    CU(cudaEventRecord(c->eval_ev[c->eval_ev_used + 1], c->stream));
-    c->eval_ev_used += 2;
+  };
+  auto step = [&](size_t dyn) -> int {
     // sharded: pair matrices go straight into every peer's exchange buffer (double-buffered by iteration parity)
     PeerTable pt; std::memset(&pt, 0, sizeof pt); pt.world = 1; pt.rank = 0;
     double* eout_local = c->d_eout.as<double>();
@@ -1269,30 +1330,11 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
     if (c->comm && c->world > 1 && !use_p2p)
       NC(ncclAllReduce(c->d_eout.p, c->d_eout.p, (size_t)EOUT * E, ncclDouble, ncclSum, c->comm, c->stream));
     w.eout = eout_local; w.peer_flags = use_p2p ? pt.flags[c->rank] : nullptr; w.world = c->world; w.xseq = xs;
-    w.seq = issued + 1;
     lm_step_kernel<<<1, STEP_THREADS, dyn, c->stream>>>(w);
     c->stats.kernel_launches += (c->n_eval_tiles ? 1 : 0) + 2;
-    ++issued;
     return MVICP_OK;
   };
-  RET(issue());
-  while (true) {
-    if (issued - seen < 2 && issued <= max_evals) RET(issue());
-    // the step kernel publishes (sequence << 1 | done) into mapped pinned memory: spin on it, no stream round trip
-    const int want = seen + 1;
-    int32_t v;
-    long spins = 0;
-    while (((v = c->h_flag[want & 7]) >> 1) != want) {
-      if ((++spins & 0xfffff) == 0 && cudaStreamQuery(c->stream) != cudaErrorNotReady) {   // kernels died or stream drained
-        v = c->h_flag[want & 7];
-        if ((v >> 1) != want) { CU(cudaGetLastError()); return fail(MVICP_ERR_CUDA, "LM step %d never reported", want); }
-        break;
-      }
-    }
-    const bool fin = (v & 1) != 0;
-    ++seen;
-    if (fin || seen > max_evals) break;
-  }
+  RET(run_steps(c, lm_step_kernel, n, max_evals, "LM", w.lay, eval, step));
   // sharded runs: every rank holds bit-identical poses (the same lm_step_kernel ran on bit-identical pair matrices), so
   // no pose exchange is needed; the NCCL-only mode still all-gathers the owners' copies (6-dof poses per outer iteration,
   // as the north-star words it) -- a few small copies that change nothing.
@@ -1312,14 +1354,8 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
       if (a >= 0) CU(cudaMemcpyAsync(c->d_poses.as<double>() + 16 * a, recvb + (size_t)16 * chunk * r, sizeof(double) * 16 * (b - a + 1), cudaMemcpyDeviceToDevice, c->stream));
     }
   }
-  CU(cudaEventRecord(c->ev[4], c->stream));
-  CU(cudaMemcpyAsync(c->h_state, c->d_state.p, sizeof st, cudaMemcpyDeviceToHost, c->stream));
-  // the host mirror follows the device: mvicp_pose_graph_knn and mvicp_set_poses' "same poses as last handed out" test read it
-  CU(cudaMemcpyAsync(c->h_poses.data(), c->d_poses.p, sizeof(double) * 16 * M, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
+  RET(read_back_solve(c, c->h_state, c->d_state.p, sizeof st));
   std::memcpy(&st, c->h_state, sizeof st);
-  CU(cudaGetLastError());
-  c->ev_lm = true;
   c->last_lm_iters = st.iteration;
   if (summary) {
     summary->termination = st.termination; summary->num_iterations = st.iteration; summary->num_successful_steps = st.n_success;
@@ -1342,26 +1378,7 @@ int mvicp_pairwise(const mvicp_config* cfg, int32_t param, int32_t cost, const d
                    int64_t n, const mvicp_lm_options* opt, double* pose16_out, mvicp_lm_summary* summary) {
   if (!src || !dst || n <= 0 || !pose16_out) return fail(MVICP_ERR_INVALID, "mvicp_pairwise: bad arguments");
   if (cost != MVICP_COST_P2P && !nor) return fail(MVICP_ERR_INVALID, "mvicp_pairwise: point-to-plane needs dst normals");
-  mvicp_ctx* c = nullptr;
-  RET(mvicp_create(cfg, &c));
-  // frame 0 = dst (constant, identity), frame 1 = src (starts at identity); edge 1 -> 0 with identity matches
-  const double* pts[2] = {dst, src}; const double* nrs[2] = {nor, nor};   // src normals are never read
-  const int64_t np[2] = {n, n};
-  int rc = mvicp_set_frames(c, 2, pts, nor ? nrs : nullptr, np);
-  const int32_t es = 1, ed = 0;
-  if (rc == MVICP_OK) rc = mvicp_set_graph(c, 1, &es, &ed);
-  if (rc == MVICP_OK) {
-    std::vector<int32_t> id(n); std::iota(id.begin(), id.end(), 0);
-    rc = mvicp_set_edge(c, 0, id.data(), id.data(), n, 1.0f);
-  }
-  if (rc == MVICP_OK) rc = mvicp_optimize(c, param, cost, 0, opt, summary);
-  std::vector<double> poses(32);
-  if (rc == MVICP_OK) rc = mvicp_get_poses(c, poses.data());
-  if (rc == MVICP_OK) std::memcpy(pose16_out, poses.data() + 16, sizeof(double) * 16);
-  const std::string keep = g_err;
-  mvicp_destroy(c);
-  g_err = keep;
-  return rc;
+  return run_pairwise(cfg, src, dst, nor, n, pose16_out, [&](mvicp_ctx* c) { return mvicp_optimize(c, param, cost, 0, opt, summary); });
 }
 
 }  // extern "C"
@@ -1394,9 +1411,7 @@ int mvicp_optimize_g2o(mvicp_ctx* c, int32_t cost, const mvicp_g2o_options* opt_
   CU(cudaSetDevice(c->device));
   const int M = c->M, E = c->E;
   c->fixed[0] = 1;   // frames[0]->fixed = true (icp-g2o.cpp:182-186)
-  bool stale = false;
-  for (int e = 0; e < E; ++e) if ((c->edge_owner[e] < 0) != (c->fixed[c->h_edges[e].src] != 0)) stale = true;
-  if (stale) RET(refresh_after_fixed_change(c));
+  RET(refresh_if_fixed_changed(c));
   // every edge with a free end carries one GICP edge per stored correspondence (an edge between fixed vertices is not active)
   const int tl = c->eval_tile_len;
   std::vector<Tile> tiles; std::vector<int32_t> tb(E + 1, 0);
@@ -1435,17 +1450,9 @@ int mvicp_optimize_g2o(mvicp_ctx* c, int32_t cost, const mvicp_g2o_options* opt_
     if (chi2_per_call) chi2_per_call[0] = 0.0;
     return MVICP_OK;
   }
-  BlockLists blk((size_t)M * M), gl(M);
-  for (int e = 0; e < E; ++e) {
-    if (!cnt[e]) continue;
-    const int s = c->h_edges[e].src, k = c->h_edges[e].dst;
-    const bool fs = c->h_col[s] >= 0, fk = c->h_col[k] >= 0;
-    if (fs) { blk[(size_t)s * M + s].push_back({e, 0}); gl[s].push_back({e, 0}); }
-    if (fs && fk) { blk[(size_t)s * M + k].push_back({e, 1}); blk[(size_t)k * M + s].push_back({e, 2}); }
-    if (fk) { blk[(size_t)k * M + k].push_back({e, 3}); gl[k].push_back({e, 1}); }
-  }
-  RET(prepare_lm(c, n));
-  RET(upload_lm_structure(c, n, blk, gl));
+  std::vector<uint8_t> active(E);
+  for (int e = 0; e < E; ++e) active[e] = cnt[e] != 0;
+  RET(build_normal_layout(c, n, active));
   c->lm_key.clear();   // the buffers now hold the g2o structure: the next mvicp_optimize rebuilds its own
   RET(c->d_g2o_state.reserve(sizeof(G2oState)));
   RET(c->d_g2o_x.reserve(sizeof(Rt) * M)); RET(c->d_g2o_ev.reserve(sizeof(Rt) * M)); RET(c->d_g2o_nop.reserve(sizeof(int32_t) * M));
@@ -1459,66 +1466,28 @@ int mvicp_optimize_g2o(mvicp_ctx* c, int32_t cost, const mvicp_g2o_options* opt_
   G2oState* dS = c->d_g2o_state.as<G2oState>();
 
   G2oWork w{};
-  w.S = dS; w.eout = c->d_eout.as<double>(); w.host_flag = c->d_flag;
-  w.x = c->d_g2o_x.as<Rt>(); w.ev = c->d_g2o_ev.as<Rt>(); w.n_oplus = c->d_g2o_nop.as<int32_t>(); w.col = c->d_col.as<int32_t>();
-  w.hb_ptr = c->d_hb_ptr.as<int32_t>(); w.hb_row = c->d_hb_row.as<int32_t>(); w.hb_col = c->d_hb_col.as<int32_t>();
-  w.hc_edge = c->d_hc_edge.as<int32_t>(); w.hc_sub = c->d_hc_sub.as<int32_t>(); w.n_hblocks = c->n_hblocks;
-  w.gb_ptr = c->d_gb_ptr.as<int32_t>(); w.gc_edge = c->d_gc_edge.as<int32_t>(); w.gc_side = c->d_gc_side.as<int32_t>();
-  w.rlast = c->d_rlast.as<int32_t>(); w.rfirst = c->d_rfirst.as<int32_t>(); w.rowbase = c->d_rowbase.as<int32_t>();
-  w.H = c->d_H.as<double>(); w.b = c->d_g.as<double>(); w.Lg = c->d_L.as<double>(); w.rhs = c->d_rhs.as<double>();
-  w.poses16 = c->d_poses.as<double>(); w.chi_calls = c->d_g2o_chi.as<double>(); w.trace = c->d_g2o_trace.as<double>();
-  const size_t l_bytes = sizeof(double) * (size_t)c->l_size;
-  const size_t vec_bytes = sizeof(double) * 3 * (size_t)(n + 1);
-  w.l_in_smem = (l_bytes + vec_bytes) <= 220 * 1024 ? 1 : 0;
-  const size_t dyn = vec_bytes + (w.l_in_smem ? l_bytes : 0);
-  CU(cudaFuncSetAttribute(g2o_step_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+  w.S = dS; w.eout = c->d_eout.as<double>();
+  w.x = c->d_g2o_x.as<Rt>(); w.ev = c->d_g2o_ev.as<Rt>(); w.n_oplus = c->d_g2o_nop.as<int32_t>();
+  w.lay = c->lay; w.lay.poses16 = c->d_poses.as<double>();
+  w.H = c->d_H.as<double>(); w.g = c->d_g.as<double>();
+  w.chi_calls = c->d_g2o_chi.as<double>(); w.trace = c->d_g2o_trace.as<double>();
 
   CU(cudaEventRecord(c->ev[3], c->stream));
   g2o_init_kernel<<<(M + 63) / 64, 64, 0, c->stream>>>(w, M);
   c->stats.kernel_launches += 1;
-  // pipelined as mvicp_optimize: the next evaluation is enqueued before the host learns whether the last one finished the
-  // solve; the kernels read what to evaluate (build or trial) from the state, and exit at once after termination
+  // the kernels read what to evaluate (build or trial) from the state
   const int64_t max_evals = (int64_t)opt.max_calls * opt.iterations_per_call * (opt.max_trials + 1) + 2;
-  for (int i = 0; i < 8; ++i) c->h_flag[i] = 0;
-  c->eval_ev_used = 0;
-  int64_t issued = 0, seen = 0;
   const double eps = opt.information_eps;
-  auto issue = [&]() -> int {
-    if ((int)c->eval_ev.size() < c->eval_ev_used + 2) { cudaEvent_t a, b; CU(cudaEventCreate(&a)); CU(cudaEventCreate(&b)); c->eval_ev.push_back(a); c->eval_ev.push_back(b); }
-    CU(cudaEventRecord(c->eval_ev[c->eval_ev_used], c->stream));
-    if (c->f32) launch_g2o_eval<true>(c, cost, nt, dS, eps); else launch_g2o_eval<false>(c, cost, nt, dS, eps);
-    CU(cudaEventRecord(c->eval_ev[c->eval_ev_used + 1], c->stream));
-    c->eval_ev_used += 2;
+  auto eval = [&]() { if (c->f32) launch_g2o_eval<true>(c, cost, nt, dS, eps); else launch_g2o_eval<false>(c, cost, nt, dS, eps); };
+  auto step = [&](size_t dyn) -> int {
     g2o_edge_kernel<<<E, EDGE_THREADS, 0, c->stream>>>(c->d_g2o_tile_begin.as<int32_t>(), c->d_partial.as<double>(), dS, c->d_eout.as<double>());
-    w.seq = (int32_t)(issued + 1);
     g2o_step_kernel<<<1, STEP_THREADS, dyn, c->stream>>>(w);
     c->stats.kernel_launches += 3;
-    ++issued;
     return MVICP_OK;
   };
-  RET(issue());
-  while (true) {
-    if (issued - seen < 2 && issued <= max_evals) RET(issue());
-    const int32_t want = (int32_t)(seen + 1);
-    int32_t v;
-    long spins = 0;
-    while (((v = c->h_flag[want & 7]) >> 1) != want) {
-      if ((++spins & 0xfffff) == 0 && cudaStreamQuery(c->stream) != cudaErrorNotReady) {
-        v = c->h_flag[want & 7];
-        if ((v >> 1) != want) { CU(cudaGetLastError()); return fail(MVICP_ERR_CUDA, "g2o step %d never reported", want); }
-        break;
-      }
-    }
-    ++seen;
-    if ((v & 1) != 0 || seen > max_evals) break;
-  }
-  CU(cudaEventRecord(c->ev[4], c->stream));
-  CU(cudaMemcpyAsync(&st, dS, sizeof st, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaMemcpyAsync(c->h_poses.data(), c->d_poses.p, sizeof(double) * 16 * M, cudaMemcpyDeviceToHost, c->stream));
-  CU(cudaStreamSynchronize(c->stream));
-  CU(cudaGetLastError());
+  RET(run_steps(c, g2o_step_kernel, n, max_evals, "g2o", w.lay, eval, step));
+  RET(read_back_solve(c, &st, dS, sizeof st));
   if (chi2_per_call) CU(cudaMemcpy(chi2_per_call, c->d_g2o_chi.p, sizeof(double) * (st.call + 1), cudaMemcpyDeviceToHost));
-  c->ev_lm = true;
   c->last_lm_iters = 1 << 20;
   c->g2o_trials = st.n_trace;
   if (summary) {
@@ -1537,26 +1506,7 @@ int mvicp_pairwise_g2o(const mvicp_config* cfg, int32_t cost, const double* src,
   mvicp_g2o_options opt;
   if (opt_in) opt = *opt_in; else { mvicp_default_g2o_options(&opt); opt.iterations_per_call = 300; }   // optimize(300), icp-g2o.cpp:72,133
   opt.max_calls = 1;
-  mvicp_ctx* c = nullptr;
-  RET(mvicp_create(cfg, &c));
-  // vertex 0 = dst (fixed at the identity), vertex 1 = src (from the identity); edge 1 -> 0 with identity matches
-  const double* pts[2] = {dst, src}; const double* nrs[2] = {nor, nor};   // src normals are never read
-  const int64_t np[2] = {n, n};
-  int rc = mvicp_set_frames(c, 2, pts, nor ? nrs : nullptr, np);
-  const int32_t es = 1, ed = 0;
-  if (rc == MVICP_OK) rc = mvicp_set_graph(c, 1, &es, &ed);
-  if (rc == MVICP_OK) {
-    std::vector<int32_t> id(n); std::iota(id.begin(), id.end(), 0);
-    rc = mvicp_set_edge(c, 0, id.data(), id.data(), n, 1.0f);
-  }
-  if (rc == MVICP_OK) rc = mvicp_optimize_g2o(c, cost, &opt, summary, nullptr);
-  std::vector<double> poses(32);
-  if (rc == MVICP_OK) rc = mvicp_get_poses(c, poses.data());
-  if (rc == MVICP_OK) std::memcpy(pose16_out, poses.data() + 16, sizeof(double) * 16);
-  const std::string keep = g_err;
-  mvicp_destroy(c);
-  g_err = keep;
-  return rc;
+  return run_pairwise(cfg, src, dst, nor, n, pose16_out, [&](mvicp_ctx* c) { return mvicp_optimize_g2o(c, cost, &opt, summary, nullptr); });
 }
 
 int mvicp_g2o_trace(mvicp_ctx* c, double* out5, int64_t capacity, int64_t* n_trials) {
