@@ -7,7 +7,9 @@ the rounding level, so equal numbers of calls and trials after that point cannot
     and chi > 1e-20 chi2_initial (below that an exact fit has been reached and chi2 is rounding noise): the same accept /
     reject decisions and lambda within 1e-9 relative;
   * the final chi2 within 1e-9 relative, the final poses within 1e-8;
-  * two runs of the engine bit-identical (poses, chi2 per call and trace)."""
+  * two runs of the engine bit-identical (poses, chi2 per call and trace);
+  * a build and a trial evaluation at the same poses give the same chi2 bits (the trace's chi after an accepted trial is its
+    tchi, after a rejected one the same chi; chi2 at the start of every call is the chi of a trace row)."""
 import numpy as np
 import pytest
 
@@ -51,6 +53,16 @@ def check_against_model(eng, pts, nor, poses, edges, fixed, cost, options=None):
         if f not in prob.col:
             assert np.array_equal(P[f], np.asarray(poses[f])), f
     assert summ["trials"] == len(trace) and summ["calls"] == len(chis) - 1
+    # a build and a trial evaluation at the same poses give the same chi2 bits (every rho compares the two): after an accepted
+    # trial the next row's chi is that trial's tchi; after a rejected one it is the same chi (the same iteration, or a rebuild
+    # at the same estimate); and chi2 at the start of every call is the chi of a row, the first of that call
+    for r in range(len(trace) - 1):
+        assert trace[r + 1, 1] == (trace[r, 2] if trace[r, 4] else trace[r, 1]), (r, trace[r], trace[r + 1])
+    r = 0
+    for c in range(len(chis) - 1):
+        while r < len(trace) and trace[r, 1] != chis[c]:
+            r += 1
+        assert r < len(trace), (c, chis[c])
     # a second run from the same start is bit-identical
     eng.set_poses(poses, fixed)
     summ2, chis2 = eng.optimize_g2o(cost, options)
