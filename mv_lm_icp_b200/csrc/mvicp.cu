@@ -750,8 +750,7 @@ template <bool F32> static int launch_correspond(mvicp_ctx* c, float thresh) {
 #define MV_KNN_ARGS c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_xf.as<EdgeXf>(), c->d_knn_tiles.as<Tile>(), \
                     c->d_corr.as<int32_t>(), c->d_d2.as<double>(), seed ? c->d_corr.as<int32_t>() : nullptr, d2max
 #define MV_KNN_TAIL sg, E, c->d_certs.as<float4>()
-    if (far && ww) knn_far_kernel<F32, true><<<c->n_knn_tiles, KNN_TILE, 0, c->stream>>>(MV_KNN_ARGS, c->d_obb.as<ObbDev>());
-    else if (far) knn_far_kernel<F32, false><<<c->n_knn_tiles, KNN_TILE, 0, c->stream>>>(MV_KNN_ARGS, c->d_obb.as<ObbDev>());
+    if (far) knn_far_kernel<F32><<<c->n_knn_tiles, KNN_TILE, 0, c->stream>>>(MV_KNN_ARGS, c->d_obb.as<ObbDev>());
     else if (cert == 2) {
       const CertTodo todo = {c->d_todo.as<int2>(), c->d_todo_n.as<unsigned int>()};
       knn_cert_kernel<F32><<<c->n_knn_tiles, KNN_TILE, 0, c->stream>>>(MV_KNN_ARGS, MV_KNN_TAIL, c->d_cert_cnt.as<unsigned long long>(), todo);

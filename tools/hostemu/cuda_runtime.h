@@ -161,6 +161,20 @@ inline unsigned __ballot_sync(unsigned, int p) {
   hostemu::yield(hostemu::AT_WARP);
   return r;
 }
+// whole-warp integer reductions (redux.sync): min / max over the lanes that have not returned
+static unsigned reduce_slot[64][32];
+template <class Op> inline unsigned hostemu_reduce(unsigned v, Op op) {
+  const int w = hostemu::cur / 32, l = hostemu::cur % 32;
+  reduce_slot[w][l] = v;
+  hostemu::yield(hostemu::AT_WARP);
+  bool first = true; unsigned r = 0;
+  for (int i = 0; i < 32; ++i)
+    if (32 * w + i < hostemu::n_threads && hostemu::fibers[32 * w + i].state != hostemu::DONE) { r = first ? reduce_slot[w][i] : op(r, reduce_slot[w][i]); first = false; }
+  hostemu::yield(hostemu::AT_WARP);
+  return r;
+}
+inline unsigned __reduce_min_sync(unsigned, unsigned v) { return hostemu_reduce(v, [](unsigned a, unsigned b) { return a < b ? a : b; }); }
+inline unsigned __reduce_max_sync(unsigned, unsigned v) { return hostemu_reduce(v, [](unsigned a, unsigned b) { return a > b ? a : b; }); }
 // sub-warp collectives (mask names the participants): modelled on the whole-warp barrier, so every lane of the warp that is
 // still alive must reach SOME warp-level barrier while the named lanes exchange -- true for the engine's uses, where the
 // lanes outside the mask wait at the __syncwarp that follows.
@@ -199,6 +213,8 @@ inline long long clock64() { return std::chrono::steady_clock::now().time_since_
 template <class T> inline T __ldg(const T* p) { return *p; }
 inline int __float_as_int(float f) { int i; std::memcpy(&i, &f, 4); return i; }
 inline float __int_as_float(int i) { float f; std::memcpy(&f, &i, 4); return f; }
+inline unsigned __float_as_uint(float f) { unsigned i; std::memcpy(&i, &f, 4); return i; }
+inline float __uint_as_float(unsigned i) { float f; std::memcpy(&f, &i, 4); return f; }
 inline long long __double_as_longlong(double d) { long long l; std::memcpy(&l, &d, 8); return l; }
 inline double __longlong_as_double(long long l) { double d; std::memcpy(&d, &l, 8); return d; }
 inline double __dmul_rn(double a, double b) { return a * b; }   // compile with -ffp-contract=off
