@@ -158,6 +158,21 @@ int mvicp_closest_point(mvicp_ctx* ctx, int32_t frame, const double query[3], in
 int mvicp_optimize(mvicp_ctx* ctx, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt,
                    mvicp_lm_summary* summary);
 
+/* Connected components of the current graph: the undirected graph the edges induce over all frames (a frame without edges is
+ * a component of its own), numbered in ascending order of their lowest frame.  *n_components, and component_of_frame[M]
+ * (nullable). */
+int mvicp_get_components(mvicp_ctx* ctx, int32_t* n_components, int32_t* component_of_frame);
+/* One independent LM solve per component, all in one pipelined loop: a batch of unrelated registrations in one context.  The
+ * lowest frame of every component is fixed (and stays fixed, as frame 0 does after mvicp_optimize; user-set flags are kept).
+ * Each component is solved exactly as mvicp_optimize would solve it in a fresh context holding only that component (its frames
+ * in ascending order, its edges in graph order, the same fixed flags and options): its own trust region, counters,
+ * termination and costs; on a connected graph the result equals mvicp_optimize's bit for bit.  Shared by the batch: the
+ * streaming tile length (from all active correspondence slots), the unit / general eval path (general if any pose is not
+ * rigid) and the storage mode.  Every frame's pose is written back.  summaries (nullable): n_components entries; a component
+ * without a free frame gets mvicp_optimize's summary for a problem without unknowns.  Sharded context: MVICP_ERR_STATE. */
+int mvicp_optimize_components(mvicp_ctx* ctx, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt,
+                              mvicp_lm_summary* summaries);
+
 /* ICP_G2O::g2oOptimizer (include/icp-g2o.h:14, icp-g2o.cpp:149-303), the --g2o path of main_multiview.cpp:158-164: one g2o
  * Edge_V_V_GICP per stored correspondence of every edge with a free end (vertex 0 = dst, vertex 1 = src), VertexSE3 poses,
  * Levenberg-Marquardt over H + lambda I (no Jacobi scaling), and the reference's outer loop of optimize(iterations_per_call)

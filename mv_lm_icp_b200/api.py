@@ -307,6 +307,24 @@ class Engine:
                                      C.byref(options) if options is not None else None, C.byref(s)))
         return s.asdict()
 
+    def components(self):
+        """Connected components of the current graph (mvicp_get_components): (n, component_of_frame), numbered in ascending
+        order of their lowest frame; a frame without edges is a component of its own."""
+        n = C.c_int32(0); comp = np.zeros(self.M, np.int32)
+        check(self._l.mvicp_get_components(self._ctx, C.byref(n), _p(comp, C.c_int32)))
+        return n.value, comp
+
+    def optimize_components(self, param=PARAM_SE3, cost=COST_P2PLANE, robust=True, options=None):
+        """One independent LM solve per connected component, all in one batched loop (mvicp_optimize_components): each
+        component ends exactly as optimize() would in an engine holding only that component.  Fixes the lowest frame of every
+        component.  Returns one summary dict per component, in component order."""
+        n = C.c_int32(0)
+        check(self._l.mvicp_get_components(self._ctx, C.byref(n), None))
+        s = (LmSummary * max(1, n.value))()
+        check(self._l.mvicp_optimize_components(self._ctx, C.c_int32(param), C.c_int32(cost), C.c_int32(int(robust)),
+                                                C.byref(options) if options is not None else None, s))
+        return [s[k].asdict() for k in range(n.value)]
+
     def icp_round(self, thresh=0.05, param=PARAM_SE3, cost=COST_P2PLANE, robust=True, options=None):
         s = LmSummary()
         check(self._l.mvicp_icp_round(self._ctx, C.c_float(thresh), C.c_int32(param), C.c_int32(cost),

@@ -51,9 +51,9 @@ template <bool F32, bool NF32, int COST>
 __global__ void __launch_bounds__(EVAL_THREADS, 2)
 lm_eval_kernel(const FrameDev* __restrict__ frames, const EdgeDev* __restrict__ edges, const Tile* __restrict__ tiles,
                int tile_len, const int32_t* __restrict__ corr, const Rt* __restrict__ frame_Rt,
-               const float* __restrict__ weight, int robust, double* __restrict__ partial, const int* __restrict__ done_flag) {
-  if (*done_flag) return;   // issued speculatively after the solve terminated
+               const float* __restrict__ weight, int robust, double* __restrict__ partial, DoneGate gate) {
   const Tile t = tiles[blockIdx.x];
+  if (gate.skip(t.edge)) return;   // issued speculatively after the solve (of this edge's component) terminated
   const EdgeDev e = edges[t.edge];
   __shared__ double sRel[12];
   __shared__ double sred[EVAL_THREADS / 32][NBLK];
@@ -240,8 +240,8 @@ __device__ __forceinline__ void edge_signal(const PeerTable& pt, int seq, unsign
 __global__ void __launch_bounds__(EDGE_THREADS)
 lm_edge_kernel(const EdgeDev* __restrict__ edges, const int32_t* __restrict__ edge_tile_begin, const double* __restrict__ partial,
                int nused, const Rt* __restrict__ frame_Rt, const double* __restrict__ K_eval, double* __restrict__ out,
-               const int* __restrict__ done_flag, PeerTable pt, int seq, unsigned int* counter) {
-  if (*done_flag) return;
+               DoneGate gate, PeerTable pt, int seq, unsigned int* counter) {
+  if (gate.skip(blockIdx.x)) return;
   const int e = blockIdx.x, tid = threadIdx.x;
   __shared__ double blk[NBLK], Q[36], AQ[36], Hcan[144], T1[144], Rt_[9];
   double* o = out + (size_t)EOUT_ * e;
@@ -386,9 +386,9 @@ template <bool F32, bool NF32, int COST>
 __global__ void __launch_bounds__(EVAL_THREADS)
 lm_eval_general_kernel(const FrameDev* __restrict__ frames, const EdgeDev* __restrict__ edges, const Tile* __restrict__ tiles,
                        int tile_len, const int32_t* __restrict__ corr, const FrameGen* __restrict__ frame_gen,
-                       const float* __restrict__ weight, int robust, int rot0, double* __restrict__ partial, const int* __restrict__ done_flag) {
-  if (*done_flag) return;
+                       const float* __restrict__ weight, int robust, int rot0, double* __restrict__ partial, DoneGate gate) {
   const Tile t = tiles[blockIdx.x];
+  if (gate.skip(t.edge)) return;
   const EdgeDev e = edges[t.edge];
   __shared__ FrameGen g2[2];                                    // [0] src frame, [1] dst frame
   __shared__ double sred[EVAL_THREADS / 32][2][GACC];
@@ -510,8 +510,8 @@ lm_eval_general_kernel(const FrameDev* __restrict__ frames, const EdgeDev* __res
 // general-path counterpart of lm_edge_kernel: the partials already are the pair matrix in the parameterisation tangent
 __global__ void __launch_bounds__(EDGE_THREADS)
 lm_edge_general_kernel(const EdgeDev* __restrict__ edges, const int32_t* __restrict__ edge_tile_begin, const double* __restrict__ partial,
-                       double* __restrict__ out, const int* __restrict__ done_flag, PeerTable pt, int seq, unsigned int* counter) {
-  if (*done_flag) return;
+                       double* __restrict__ out, DoneGate gate, PeerTable pt, int seq, unsigned int* counter) {
+  if (gate.skip(blockIdx.x)) return;
   const int e = blockIdx.x, tid = threadIdx.x;
   __shared__ double blk[GBLK];
   double* o = out + (size_t)EOUT_ * e;

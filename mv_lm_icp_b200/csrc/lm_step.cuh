@@ -58,6 +58,18 @@ struct LmWork {
   long long* prof;           // development aid (MVICP_STEP_PROFILE=1): clock64() stamps of the last solving launch, else null
 };
 
+// One LM problem as the state machine sees it: the whole graph (lm_step_kernel: frame and edge null, the layout and the dense
+// arrays of LmWork), or one connected component (lm_step_components_kernel).  Local frame f is frame frame[f] of the graph
+// (ascending), local edge e is edge edge[e] (graph order); the layout's columns, col[] and gb_ptr[] are over local frames, its
+// gather lists name graph edges.  x, cand, Rt_eval, K_eval, G_eval and the poses stay indexed by graph frame.
+struct LmProblem {
+  LmState* S;
+  const int32_t* frame;      // [S->M]
+  const int32_t* edge;       // [S->E]
+  NormalLayout lay;          // (poses16, host_flag and seq are LmWork's)
+  double *H, *g, *Hc, *gc, *scale, *diag, *step;
+};
+
 __device__ __forceinline__ double block_sum(double v, double* red) {
   __syncthreads();
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -105,14 +117,15 @@ __device__ __forceinline__ void gather_gradient(const NormalLayout& l, const dou
     g[l.col[f] + i] = s;
   }
 }
-// Total cost: edges summed in a fixed order (thread t takes edges t, t + T, ...; then the block tree) -- the same on every rank
-__device__ __forceinline__ double edge_cost_sum(const double* eout, int E, double* red) {
+// Total cost: edges summed in a fixed order (thread t takes edges t, t + T, ...; then the block tree) -- the same on every rank.
+// edge (nullable): the problem's local edge list; the order is over local edges, so a component sums as a graph of its own would.
+__device__ __forceinline__ double edge_cost_sum(const double* eout, int E, double* red, const int32_t* edge = nullptr) {
   double s = 0.0;
-  for (int e = threadIdx.x; e < E; e += blockDim.x) s += eout[(size_t)EOUT * e + 156];
+  for (int e = threadIdx.x; e < E; e += blockDim.x) s += eout[(size_t)EOUT * (edge ? edge[e] : e) + 156];
   return block_sum(s, red);
 }
 // A step kernel works on a shared-memory copy of its state (dozens of dependent scalar reads per step) and writes it back once
-// at the end; nobody else touches the state while the kernel runs
+// at the end; nobody else touches the state while the kernel runs (lm_step_components_kernel stages its LmProblem the same way)
 template <typename State> __device__ __forceinline__ void copy_state(State* dst, const State* src) {
   for (int i = threadIdx.x; i < (int)(sizeof(State) / sizeof(int32_t)); i += blockDim.x)
     reinterpret_cast<int32_t*>(dst)[i] = reinterpret_cast<const int32_t*>(src)[i];
@@ -307,18 +320,24 @@ __device__ bool chol_solve(double* L, const int32_t* __restrict__ rowbase, int n
   return true;
 }
 
-__global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
+// ---- the LM trust-region state machine: one step of one problem, one CTA -----------------------------------------------
+// COMP = false: the whole graph, which publishes the step into the ring itself; COMP = true: one connected component, whose
+// kernel publishes once every component's CTA has stepped.  Every loop over frames, edges and columns runs over the problem's
+// LOCAL indices, so a component's reductions are associated exactly as in a context that holds only that component.
+template <bool COMP>
+__device__ __forceinline__ void lm_step_body(const LmWork& w, const LmProblem& p) {
   extern __shared__ double smem[];
   __shared__ double red[40];
   __shared__ int s_flag;
-  if (w.S->done) { if (threadIdx.x == 0) publish_step(w.lay, true); return; }
+  if (p.S->done) { if (!COMP && threadIdx.x == 0) publish_step(w.lay, true); return; }
   const int tid = threadIdx.x, T = blockDim.x;
   __shared__ LmState s_state;
-  copy_state(&s_state, w.S);
+  copy_state(&s_state, p.S);
   LmState* S = &s_state;
   const int n = S->n, M = S->M, E = S->E, param = S->param;
-  const NormalLayout& lay = w.lay;
-  long long* prof = w.prof ? w.prof + 16 * (lay.seq & 3) : nullptr;   // one row of stamps per launch, the last four launches kept
+  const NormalLayout& lay = p.lay;
+  auto gf = [&](int f) { return COMP ? p.frame[f] : f; };   // local frame -> frame of the graph
+  long long* prof = w.prof ? w.prof + 16 * (w.lay.seq & 3) : nullptr;   // one row of stamps per launch, the last four launches kept
 #define MV_STAMP(i) do { if (prof && tid == 0) prof[i] = clock64(); } while (0)
   MV_STAMP(0);
   if (w.peer_flags) {   // wait until every rank's edge kernel has delivered this iteration's pair matrices
@@ -335,10 +354,10 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
   double* L = lay.l_in_smem ? smem + 3 * (S->n + 1) : lay.Lg;
 
   // ================= 1. gather the per-edge pair matrices (lm_edge_kernel) into Hc, gc; total cost ===================
-  gather_blocks(lay, w.eout, n, w.Hc);
-  gather_gradient(lay, w.eout, M, w.gc);
+  gather_blocks(lay, w.eout, n, p.Hc);
+  gather_gradient(lay, w.eout, M, p.gc);
   __syncthreads();
-  const double eval_cost = edge_cost_sum(w.eout, E, red);
+  const double eval_cost = edge_cost_sum(w.eout, E, red, COMP ? p.edge : nullptr);
 
   MV_STAMP(1);
   // ================= 2. accept / reject / terminate =================================================
@@ -381,21 +400,21 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
     for (int idx = tid; idx < lay.n_hblocks * 36; idx += T) {
       const int b = idx / 36, r = idx - 36 * b, i = r / 6, j = r - 6 * i;
       const size_t at = (size_t)(lay.hb_row[b] + i) * n + lay.hb_col[b] + j;
-      w.H[at] = w.Hc[at];
+      p.H[at] = p.Hc[at];
     }
-    for (int idx = tid; idx < n; idx += T) w.g[idx] = w.gc[idx];
-    for (int idx = tid; idx < M * 7; idx += T) w.x[idx] = w.cand[idx];
+    for (int idx = tid; idx < n; idx += T) p.g[idx] = p.gc[idx];
+    for (int idx = tid; idx < M * 7; idx += T) { const int at = COMP ? 7 * gf(idx / 7) + idx % 7 : idx; w.x[at] = w.cand[at]; }
     __syncthreads();
     if (S->phase == 0)
-      for (int j = tid; j < n; j += T) w.scale[j] = S->opt.jacobi_scaling ? 1.0 / (1.0 + sqrt(w.H[(size_t)j * n + j])) : 1.0;
+      for (int j = tid; j < n; j += T) p.scale[j] = S->opt.jacobi_scaling ? 1.0 / (1.0 + sqrt(p.H[(size_t)j * n + j])) : 1.0;
     // x_norm over the free blocks, and the gradient test |x - Plus(x, -g)|_inf
     double xs = 0.0, gm = 0.0;
     for (int f = tid; f < M; f += T) {
       if (lay.col[f] < 0) continue;
       const int G = S->G;
       double xf[7], ng[6], xp[7];
-      for (int i = 0; i < G; ++i) { xf[i] = w.x[7 * f + i]; xs += xf[i] * xf[i]; }
-      for (int i = 0; i < 6; ++i) ng[i] = -w.g[lay.col[f] + i];
+      for (int i = 0; i < G; ++i) { xf[i] = w.x[7 * gf(f) + i]; xs += xf[i] * xf[i]; }
+      for (int i = 0; i < 6; ++i) ng[i] = -p.g[lay.col[f] + i];
       param_plus(param, xf, ng, xp);
       for (int i = 0; i < G; ++i) gm = fmax(gm, fabs(xf[i] - xp[i]));
     }
@@ -424,20 +443,20 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
     __syncthreads();
     if (!reuse)
       for (int j = tid; j < n; j += T) {
-        const double d = w.scale[j] * w.scale[j] * w.H[(size_t)j * n + j];
-        w.diag[j] = fmin(fmax(d, S->opt.min_lm_diagonal), S->opt.max_lm_diagonal);
+        const double d = p.scale[j] * p.scale[j] * p.H[(size_t)j * n + j];
+        p.diag[j] = fmin(fmax(d, S->opt.min_lm_diagonal), S->opt.max_lm_diagonal);
       }
     __syncthreads();
     for (int i = tid >> 5; i < n; i += T >> 5) {          // one warp per row, only the row's profile (see chol_solve)
-      const double si = w.scale[i];
+      const double si = p.scale[i];
       const int rbi = lay.rowbase[i];
       for (int j = lay.rfirst[i] + (tid & 31); j <= i; j += 32) {
-        double v = si * w.H[(size_t)i * n + j] * w.scale[j];
-        if (i == j) { const double ldg = sqrt(w.diag[i] / radius); v += ldg * ldg; }
+        double v = si * p.H[(size_t)i * n + j] * p.scale[j];
+        if (i == j) { const double ldg = sqrt(p.diag[i] / radius); v += ldg * ldg; }
         L[rbi + j] = v;
       }
     }
-    { const int rbn = lay.rowbase[n]; for (int j = tid; j < n; j += T) L[rbn + j] = w.scale[j] * w.g[j]; }
+    { const int rbn = lay.rowbase[n]; for (int j = tid; j < n; j += T) L[rbn + j] = p.scale[j] * p.g[j]; }
     __syncthreads();
     MV_STAMP(3);
     bool ok = chol_solve(L, lay.rowbase, n, colj, dg, lay.rhs, lay.rlast, lay.rfirst, prof);
@@ -448,14 +467,14 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
     ok = ok && (bad == 0.0);
     double mcc = 0.0;
     if (ok) {
-      for (int j = tid; j < n; j += T) w.step[j] = -lay.rhs[j];
+      for (int j = tid; j < n; j += T) p.step[j] = -lay.rhs[j];
       __syncthreads();
       // model_cost_change = -(J s).(r + J s / 2) = -s.g~ - 1/2 s^T H~ s; with (H~ + D^2) y = g~ and s = -y this is
       // 1/2 (y.g~ + sum D_i^2 y_i^2): O(n) instead of O(n^2)
       double acc = 0.0;
       for (int i = tid; i < n; i += T) {
         const double y = lay.rhs[i];
-        acc += 0.5 * (y * w.scale[i] * w.g[i] + (w.diag[i] / radius) * y * y);
+        acc += 0.5 * (y * p.scale[i] * p.g[i] + (p.diag[i] / radius) * y * y);
       }
       mcc = block_sum(acc, red);
     }
@@ -474,20 +493,20 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
     // candidate = Plus(x, step * scale) per free frame; step norm in the ambient space
     double sn = 0.0;
     for (int f = tid; f < M; f += T) {
-      const int G = S->G;
+      const int G = S->G, g_f = gf(f);
       double xf[7], d[6], xp[7] = {0, 0, 0, 0, 0, 0, 0};
-      for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * f + i];
+      for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * g_f + i];
       if (lay.col[f] >= 0) {
-        for (int i = 0; i < 6; ++i) d[i] = w.step[lay.col[f] + i] * w.scale[lay.col[f] + i];
+        for (int i = 0; i < 6; ++i) d[i] = p.step[lay.col[f] + i] * p.scale[lay.col[f] + i];
         param_plus(param, xf, d, xp);
         for (int i = 0; i < G; ++i) sn += (xf[i] - xp[i]) * (xf[i] - xp[i]);
       } else for (int i = 0; i < 7; ++i) xp[i] = xf[i];
-      for (int i = 0; i < 7; ++i) w.cand[7 * f + i] = xp[i];
+      for (int i = 0; i < 7; ++i) w.cand[7 * g_f + i] = xp[i];
       Rt a; Rt_of_param(param, xp, &a);
-      w.Rt_eval[f] = a;
+      w.Rt_eval[g_f] = a;
       double K[36]; tangent_map(param, xp, &a, K);
-      for (int i = 0; i < 36; ++i) w.K_eval[36 * f + i] = K[i];
-      if (w.G_eval && param != PARAM_AA) frame_general(param, xp, &w.G_eval[f]);
+      for (int i = 0; i < 36; ++i) w.K_eval[36 * g_f + i] = K[i];
+      if (w.G_eval && param != PARAM_AA) frame_general(param, xp, &w.G_eval[g_f]);
     }
     sn = block_sum(sn, red);
     MV_STAMP(5);
@@ -499,16 +518,40 @@ __global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
   // ================= 4. on termination: write every frame's pose back (icp-ceres.cpp:318-322,392-394,472-474)
   if (S->done) {
     for (int f = tid; f < M; f += T) {
-      double xf[7]; for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * f + i];
-      pose_of_param(param, xf, lay.poses16 + 16 * f);
+      double xf[7]; for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * gf(f) + i];
+      pose_of_param(param, xf, w.lay.poses16 + 16 * gf(f));
     }
   }
   __syncthreads();
-  copy_state(w.S, &s_state);
+  copy_state(p.S, &s_state);
   MV_STAMP(6);
-  if (tid == 0) publish_step(lay, S->done);
+  if (!COMP && tid == 0) publish_step(w.lay, S->done);
   MV_STAMP(7);
 #undef MV_STAMP
+}
+
+__global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
+  const LmProblem p{w.S, nullptr, nullptr, w.lay, w.H, w.g, w.Hc, w.gc, w.scale, w.diag, w.step};
+  lm_step_body<false>(w, p);
+}
+
+// One CTA per connected component (probs[blockIdx.x]), each stepping its own problem.  Every CTA takes a ticket when its step is
+// written; the last one publishes (sequence << 1) | (every component done) into the ring and resets the ticket for the next
+// launch.  The problem's view is staged in shared memory once per CTA, not copied into every thread.
+__global__ void __launch_bounds__(STEP_THREADS) lm_step_components_kernel(LmWork w, const LmProblem* __restrict__ probs, unsigned int* ticket) {
+  __shared__ LmProblem s_prob;
+  copy_state(&s_prob, probs + blockIdx.x);
+  lm_step_body<true>(w, s_prob);
+  __shared__ int s_last;
+  __syncthreads();
+  if (threadIdx.x == 0) { __threadfence(); s_last = atomicAdd(ticket, 1u) == gridDim.x - 1; }
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  int open = 0;
+  for (int k = threadIdx.x; k < (int)gridDim.x; k += blockDim.x) open |= *(volatile const int*)&probs[k].S->done == 0;
+  open = __syncthreads_count(open);
+  if (threadIdx.x == 0) { *ticket = 0u; publish_step(w.lay, open == 0); }
 }
 
 }  // namespace mv

@@ -128,6 +128,13 @@ struct mvicp_ctx {
   void* h_state = nullptr;     // pinned staging of LmState
   volatile int32_t* h_flag = nullptr; volatile int32_t* d_flag = nullptr;   // mapped pinned ring written by lm_step_kernel
   std::vector<uint8_t> lm_key; uint32_t graph_gen = 0;
+  // per-component solve (mvicp_optimize_components): its own layouts, dense arrays and states, cached under cmp_key
+  DevBuf d_cmp_i32, d_cmp_f64, d_cmp_prob, d_cmp_state, d_cmp_ticket;
+  std::vector<uint8_t> cmp_key;
+  std::vector<int32_t> cmp_of_frame;     // component of every frame (numbered by lowest frame)
+  std::vector<int32_t> cmp_prob;         // component -> its problem (the components with a free frame), or -1
+  std::vector<int32_t> cmp_M, cmp_E, cmp_n;   // frames, edges and unknowns of every problem
+  int n_cmp = 0, n_prob = 0; size_t cmp_dyn = 0, cmp_edge_map = 0;   // dynamic shared memory of the step; edge -> problem in d_cmp_i32
   // g2o solve (g2o.cuh); shares the normal-matrix buffers above and clears lm_key when it has used them
   DevBuf d_g2o_state, d_g2o_x, d_g2o_ev, d_g2o_nop, d_g2o_chi, d_g2o_trace, d_g2o_tiles, d_g2o_tile_begin, d_g2o_cnt;
   int64_t g2o_trials = 0;
@@ -1059,53 +1066,77 @@ int mvicp_closest_points_device(mvicp_ctx* c, int32_t frame, const double* q, in
 // matrix's ss / sk / ks / kk sub-blocks into blocks (s, s) / (s, k) / (k, s) / (k, k) and its (e, side) pair gradient into frame
 // s's / k's gradient, wherever those ends have a column.  Uploads the gather lists, the envelope and the skyline layout of the
 // factor, and zeroes the dense normal matrix.
-static int build_normal_layout(mvicp_ctx* c, int n, const std::vector<uint8_t>& active) {
-  const int M = c->M, E = c->E;
+//
+// plan_normal_layout is the host half for one problem: `frames` (ascending) are its frames, local frame i being frames[i], and
+// `edges` its edges in graph order; c->h_col holds the local columns (n of them).  The gather lists name graph edges.
+struct LayoutPlan {
+  std::vector<int32_t> col, hb_ptr{0}, hb_row, hb_col, hc_edge, hc_sub, gb_ptr{0}, gc_edge, gc_side, rlast, rfirst, rowbase;
+  int64_t l_size = 0;        // doubles of the factor's skyline storage (row profiles + rhs row)
+};
+static int plan_normal_layout(const mvicp_ctx* c, const std::vector<int32_t>& frames, const std::vector<int32_t>& edges, int n,
+                              const std::vector<uint8_t>& active, LayoutPlan& p) {
+  const int M = (int)frames.size();
+  std::vector<int32_t> loc(c->M, -1);
+  for (int i = 0; i < M; ++i) loc[frames[i]] = i;
   std::vector<std::vector<std::pair<int, int>>> blk((size_t)M * M), gl(M);
-  for (int e = 0; e < E; ++e) {
+  for (const int e : edges) {
     if (!active[e]) continue;
-    const int s = c->h_edges[e].src, k = c->h_edges[e].dst;
-    const bool fs = c->h_col[s] >= 0, fk = c->h_col[k] >= 0;
+    const int s = loc[c->h_edges[e].src], k = loc[c->h_edges[e].dst];
+    const bool fs = c->h_col[frames[s]] >= 0, fk = c->h_col[frames[k]] >= 0;
     if (fs) { blk[(size_t)s * M + s].push_back({e, 0}); gl[s].push_back({e, 0}); }
     if (fs && fk) { blk[(size_t)s * M + k].push_back({e, 1}); blk[(size_t)k * M + s].push_back({e, 2}); }
     if (fk) { blk[(size_t)k * M + k].push_back({e, 3}); gl[k].push_back({e, 1}); }
   }
-  std::vector<int32_t> hb_ptr{0}, hb_row, hb_col, hc_edge, hc_sub, gb_ptr{0}, gc_edge, gc_side;
+  p.col.resize(M);
+  for (int i = 0; i < M; ++i) p.col[i] = c->h_col[frames[i]];
   for (int r = 0; r < M; ++r)
     for (int q = 0; q < M; ++q) {
       const auto& l = blk[(size_t)r * M + q];
       if (l.empty()) continue;
-      hb_row.push_back(c->h_col[r]); hb_col.push_back(c->h_col[q]);
-      for (auto& pr : l) { hc_edge.push_back(pr.first); hc_sub.push_back(pr.second); }
-      hb_ptr.push_back((int32_t)hc_edge.size());
+      p.hb_row.push_back(p.col[r]); p.hb_col.push_back(p.col[q]);
+      for (auto& pr : l) { p.hc_edge.push_back(pr.first); p.hc_sub.push_back(pr.second); }
+      p.hb_ptr.push_back((int32_t)p.hc_edge.size());
     }
-  for (int f = 0; f < M; ++f) { for (auto& pr : gl[f]) { gc_edge.push_back(pr.first); gc_side.push_back(pr.second); } gb_ptr.push_back((int32_t)gc_edge.size()); }
-  const int n_hblocks = (int)hb_row.size();
+  for (int f = 0; f < M; ++f) { for (auto& pr : gl[f]) { p.gc_edge.push_back(pr.first); p.gc_side.push_back(pr.second); } p.gb_ptr.push_back((int32_t)p.gc_edge.size()); }
+  const int n_hblocks = (int)p.hb_row.size();
   // envelope: first structurally non-zero column of every row, and the last row that reaches column j
-  std::vector<int32_t> rfirst(n), rlast(n);
+  std::vector<int32_t>& rfirst = p.rfirst; std::vector<int32_t>& rlast = p.rlast;
+  rfirst.resize(n); rlast.resize(n);
   for (int r = 0; r < n; ++r) rfirst[r] = (r / 6) * 6;
   for (int b = 0; b < n_hblocks; ++b)
-    if (hb_col[b] < hb_row[b]) for (int i = 0; i < 6; ++i) rfirst[hb_row[b] + i] = std::min(rfirst[hb_row[b] + i], hb_col[b]);
+    if (p.hb_col[b] < p.hb_row[b]) for (int i = 0; i < 6; ++i) rfirst[p.hb_row[b] + i] = std::min(rfirst[p.hb_row[b] + i], p.hb_col[b]);
   for (int j = 0; j < n; ++j) { rlast[j] = j; }
   for (int r = 0; r < n; ++r) for (int j = rfirst[r]; j <= r; ++j) rlast[j] = std::max(rlast[j], r);
   for (int j = 1; j < n; ++j) rlast[j] = std::max(rlast[j], rlast[j - 1]);   // monotone (fill-in stays inside)
+  // skyline storage of the Cholesky factor: row r keeps columns rfirst[r]..r, the rhs row all n
+  p.rowbase.resize(n + 1); int64_t at = 0;
+  for (int r = 0; r < n; ++r) { p.rowbase[r] = (int32_t)(at - rfirst[r]); at += r - rfirst[r] + 1; }
+  p.rowbase[n] = (int32_t)at; at += n;
+  if (at > INT32_MAX) return fail(MVICP_ERR_INVALID, "normal matrix too large");
+  p.l_size = at;
+  return MVICP_OK;
+}
+
+static int build_normal_layout(mvicp_ctx* c, int n, const std::vector<uint8_t>& active) {
+  const int E = c->E;
+  std::vector<int32_t> frames(c->M), edges(E);
+  std::iota(frames.begin(), frames.end(), 0); std::iota(edges.begin(), edges.end(), 0);
+  LayoutPlan pl;
+  RET(plan_normal_layout(c, frames, edges, n, active, pl));
+  const int n_hblocks = (int)pl.hb_row.size();
   auto up = [&](DevBuf& b, const std::vector<int32_t>& v) -> int {
     RET(b.reserve(sizeof(int32_t) * std::max<size_t>(1, v.size())));
     if (!v.empty()) CU(cudaMemcpyAsync(b.p, v.data(), sizeof(int32_t) * v.size(), cudaMemcpyHostToDevice, c->stream));
     return MVICP_OK;
   };
-  RET(up(c->d_hb_ptr, hb_ptr)); RET(up(c->d_hb_row, hb_row)); RET(up(c->d_hb_col, hb_col)); RET(up(c->d_hc_edge, hc_edge));
-  RET(up(c->d_hc_sub, hc_sub)); RET(up(c->d_gb_ptr, gb_ptr)); RET(up(c->d_gc_edge, gc_edge)); RET(up(c->d_gc_side, gc_side));
-  RET(up(c->d_col, c->h_col));
-  RET(up(c->d_rlast, rlast)); RET(up(c->d_rfirst, rfirst));
-  // skyline storage of the Cholesky factor: row r keeps columns rfirst[r]..r, the rhs row all n
-  std::vector<int32_t> rowbase(n + 1); int64_t at = 0;
-  for (int r = 0; r < n; ++r) { rowbase[r] = (int32_t)(at - rfirst[r]); at += r - rfirst[r] + 1; }
-  rowbase[n] = (int32_t)at; at += n;
-  if (at > INT32_MAX) return fail(MVICP_ERR_INVALID, "normal matrix too large");
+  RET(up(c->d_hb_ptr, pl.hb_ptr)); RET(up(c->d_hb_row, pl.hb_row)); RET(up(c->d_hb_col, pl.hb_col)); RET(up(c->d_hc_edge, pl.hc_edge));
+  RET(up(c->d_hc_sub, pl.hc_sub)); RET(up(c->d_gb_ptr, pl.gb_ptr)); RET(up(c->d_gc_edge, pl.gc_edge)); RET(up(c->d_gc_side, pl.gc_side));
+  RET(up(c->d_col, pl.col));
+  RET(up(c->d_rlast, pl.rlast)); RET(up(c->d_rfirst, pl.rfirst));
+  const int64_t at = pl.l_size;
   c->l_size = at;
   RET(c->d_L.reserve(sizeof(double) * (size_t)at));
-  RET(up(c->d_rowbase, rowbase));
+  RET(up(c->d_rowbase, pl.rowbase));
   RET(c->d_H.reserve(sizeof(double) * n * n)); RET(c->d_g.reserve(sizeof(double) * n)); RET(c->d_rhs.reserve(sizeof(double) * n));
   RET(c->d_eout.reserve(sizeof(double) * EOUT * E));
   // the step kernels write only the listed blocks of the dense normal matrix; everything else stays zero from here
@@ -1121,30 +1152,30 @@ static int build_normal_layout(mvicp_ctx* c, int n, const std::vector<uint8_t>& 
   return MVICP_OK;
 }
 }  // extern "C"
-template <bool F32> static void launch_eval(mvicp_ctx* c, int cost, int robust, const int* done_flag) {
+template <bool F32> static void launch_eval(mvicp_ctx* c, int cost, int robust, DoneGate gate) {
   const int nt = c->n_eval_tiles;
   if (!nt) return;
 #define MV_EVAL(NF, COSTK)                                                                                       \
   lm_eval_kernel<F32, NF, COSTK><<<nt, EVAL_THREADS, 0, c->stream>>>(                                            \
       c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_eval_tiles.as<Tile>(), c->eval_tile_len,       \
-      c->d_corr.as<int32_t>(), c->d_Rt.as<Rt>(), c->d_weight.as<float>(), robust, c->d_partial.as<double>(), done_flag)
+      c->d_corr.as<int32_t>(), c->d_Rt.as<Rt>(), c->d_weight.as<float>(), robust, c->d_partial.as<double>(), gate)
 #define MV_EVALC(NF) { if (cost == COST_P2P) MV_EVAL(NF, COST_P2P); else if (cost == COST_P2PLANE) MV_EVAL(NF, COST_P2PLANE); else MV_EVAL(NF, COST_MIXED); }
   if (F32 && c->nor_f32) MV_EVALC(F32) else MV_EVALC(false)
 #undef MV_EVALC
 #undef MV_EVAL
 }
 
-template <bool F32> static void launch_eval_general(mvicp_ctx* c, int param, int cost, int robust, const int* done_flag) {
+template <bool F32> static void launch_eval_general(mvicp_ctx* c, int param, int cost, int robust, DoneGate gate) {
   const int rot0 = param == PARAM_QUAT ? 0 : 3;   // tangent order: quaternion (rotation, translation), SE3 (translation, rotation)
   const int nt = c->n_eval_tiles;
   if (!nt) return;
 #define MV_EVALG(COSTK)                                                                                          \
   if (F32 && c->nor_f32) lm_eval_general_kernel<F32, F32, COSTK><<<nt, EVAL_THREADS, 0, c->stream>>>(        \
       c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_eval_tiles.as<Tile>(), c->eval_tile_len,       \
-      c->d_corr.as<int32_t>(), c->d_gen.as<FrameGen>(), c->d_weight.as<float>(), robust, rot0, c->d_partial.as<double>(), done_flag); \
+      c->d_corr.as<int32_t>(), c->d_gen.as<FrameGen>(), c->d_weight.as<float>(), robust, rot0, c->d_partial.as<double>(), gate); \
   else lm_eval_general_kernel<F32, false, COSTK><<<nt, EVAL_THREADS, 0, c->stream>>>(                        \
       c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_eval_tiles.as<Tile>(), c->eval_tile_len,       \
-      c->d_corr.as<int32_t>(), c->d_gen.as<FrameGen>(), c->d_weight.as<float>(), robust, rot0, c->d_partial.as<double>(), done_flag)
+      c->d_corr.as<int32_t>(), c->d_gen.as<FrameGen>(), c->d_weight.as<float>(), robust, rot0, c->d_partial.as<double>(), gate)
   if (cost == COST_P2P) { MV_EVALG(COST_P2P); } else if (cost == COST_P2PLANE) { MV_EVALG(COST_P2PLANE); } else { MV_EVALG(COST_MIXED); }
 #undef MV_EVALG
 }
@@ -1242,6 +1273,14 @@ static int run_pairwise(const mvicp_config* cfg, const double* src, const double
   return rc;
 }
 
+static void summary_of_state(const LmState& st, mvicp_lm_summary* s) {
+  s->termination = st.termination; s->num_iterations = st.iteration; s->num_successful_steps = st.n_success;
+  s->num_evaluations = st.n_evals; s->num_linear_solves = st.n_solves; s->reserved = 0;
+  s->initial_cost = st.initial_cost; s->final_cost = st.x_cost;
+}
+// the summary of a solve without unknowns ("nothing to optimise")
+static void summary_no_unknowns(mvicp_lm_summary* s) { std::memset(s, 0, sizeof *s); s->termination = MVICP_TERM_GRADIENT_TOLERANCE; }
+
 extern "C" {
 int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt_in, mvicp_lm_summary* summary) {
   if (!c || !c->M || !c->E) return fail(MVICP_ERR_STATE, "mvicp_optimize: frames and graph must be set first");
@@ -1256,7 +1295,7 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
   c->n_free = n / 6;
   mvicp_lm_options opt; if (opt_in) opt = *opt_in; else mvicp_default_lm_options(&opt);
   if (n == 0) {   // nothing to optimise; still "writes the poses back"
-    if (summary) { std::memset(summary, 0, sizeof *summary); summary->termination = MVICP_TERM_GRADIENT_TOLERANCE; }
+    if (summary) summary_no_unknowns(summary);
     return MVICP_OK;
   }
   RET(refresh_if_fixed_changed(c));
@@ -1297,7 +1336,7 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
   c->stats.kernel_launches += 1;
   const int max_evals = opt.max_num_iterations + 2;
   const bool use_p2p = c->comm && c->world > 1 && c->p2p_ok && E <= mvicp_ctx::X_ECAP;
-  const int* done_flag = &w.S->done;
+  const DoneGate done_flag{&w.S->done, nullptr, 0};
   auto eval = [&]() {
     if (general) { if (c->f32) launch_eval_general<true>(c, param, cost, st.robust, done_flag); else launch_eval_general<false>(c, param, cost, st.robust, done_flag); }
     else if (c->f32) launch_eval<true>(c, cost, st.robust, done_flag); else launch_eval<false>(c, cost, st.robust, done_flag);
@@ -1356,15 +1395,212 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
   RET(read_back_solve(c, c->h_state, c->d_state.p, sizeof st));
   std::memcpy(&st, c->h_state, sizeof st);
   c->last_lm_iters = st.iteration;
-  if (summary) {
-    summary->termination = st.termination; summary->num_iterations = st.iteration; summary->num_successful_steps = st.n_success;
-    summary->num_evaluations = st.n_evals; summary->num_linear_solves = st.n_solves; summary->reserved = 0;
-    summary->initial_cost = st.initial_cost; summary->final_cost = st.x_cost;
-  }
+  if (summary) summary_of_state(st, summary);
   if (st.nonrigid == 2) return fail(MVICP_ERR_NCCL, "a peer rank never delivered its pair matrices (peer-memory exchange timed out)");
   if (st.nonrigid && !general)   // cannot happen after mvicp_set_poses; guards poses that reached the device another way
     return fail(MVICP_ERR_NONRIGID, "a pose's quaternion is not unit (non-rigid Isometry) but the unit-quaternion LM path was run");
   if (!st.done) return fail(MVICP_ERR_STATE, "LM loop did not terminate within %d evaluations", max_evals);
+  return MVICP_OK;
+}
+
+}  // extern "C"
+// ---- one LM problem per connected component (mvicp_optimize_components) ---------------------------------------------
+// Connected components of the undirected graph the edges induce over all frames, numbered in ascending order of their lowest
+// frame: the root of every union-find tree is its lowest frame, so a frame's component is known once its root's is.
+static int graph_components(const mvicp_ctx* c, std::vector<int32_t>& comp) {
+  std::vector<int32_t> up(c->M);
+  std::iota(up.begin(), up.end(), 0);
+  auto root = [&](int f) { while (up[f] != f) f = up[f] = up[up[f]]; return f; };
+  for (const EdgeDev& e : c->h_edges) {
+    const int a = root(e.src), b = root(e.dst);
+    if (a != b) up[std::max(a, b)] = std::min(a, b);
+  }
+  comp.assign(c->M, -1);
+  int n = 0;
+  for (int f = 0; f < c->M; ++f) { const int r = root(f); comp[f] = r == f ? n++ : comp[r]; }
+  return n;
+}
+
+// The layouts of every component with a free frame (a "problem"), each built as plan_normal_layout builds a whole graph's, and
+// uploaded end to end: one int32 buffer (frame and edge lists, gather lists, envelopes, skylines, then the edge -> problem map),
+// one fp64 buffer (per problem H, Hc | g, gc, scale, diag, step, rhs | factor; Sigma n^2, not (Sigma n)^2), the LmProblem views.
+static int build_component_layouts(mvicp_ctx* c, const std::vector<uint8_t>& key) {
+  const int M = c->M, E = c->E;
+  const int K = c->n_cmp = graph_components(c, c->cmp_of_frame);
+  std::vector<std::vector<int32_t>> fr(K), ed(K);
+  for (int f = 0; f < M; ++f) fr[c->cmp_of_frame[f]].push_back(f);
+  for (int e = 0; e < E; ++e) ed[c->cmp_of_frame[c->h_edges[e].src]].push_back(e);
+  std::vector<uint8_t> active(E);
+  for (int e = 0; e < E; ++e) active[e] = !c->fixed[c->h_edges[e].src];
+  c->h_col.assign(M, -1);
+  c->cmp_prob.assign(K, -1); c->cmp_M.clear(); c->cmp_E.clear(); c->cmp_n.clear();
+  std::vector<LayoutPlan> plans; std::vector<int32_t> pc;   // per problem: layout, component
+  for (int k = 0; k < K; ++k) {
+    int n = 0;
+    for (int f : fr[k]) if (!c->fixed[f]) { c->h_col[f] = n; n += 6; }
+    if (!n) continue;
+    c->cmp_prob[k] = (int32_t)plans.size();
+    plans.emplace_back();
+    RET(plan_normal_layout(c, fr[k], ed[k], n, active, plans.back()));
+    pc.push_back(k); c->cmp_n.push_back(n);
+    c->cmp_M.push_back((int32_t)fr[k].size()); c->cmp_E.push_back((int32_t)ed[k].size());
+  }
+  const int P = c->n_prob = (int)plans.size();
+  if (!P) { c->cmp_key = key; return MVICP_OK; }
+  std::vector<int32_t> blob;
+  auto put = [&](const std::vector<int32_t>& v) { const size_t o = blob.size(); blob.insert(blob.end(), v.begin(), v.end()); return o; };
+  struct Off { size_t frame, edge, col, hb_ptr, hb_row, hb_col, hc_edge, hc_sub, gb_ptr, gc_edge, gc_side, rlast, rfirst, rowbase; };
+  std::vector<Off> io(P);
+  for (int q = 0; q < P; ++q) {
+    const LayoutPlan& pl = plans[q];
+    io[q] = Off{put(fr[pc[q]]), put(ed[pc[q]]), put(pl.col), put(pl.hb_ptr), put(pl.hb_row), put(pl.hb_col), put(pl.hc_edge), put(pl.hc_sub),
+                put(pl.gb_ptr), put(pl.gc_edge), put(pl.gc_side), put(pl.rlast), put(pl.rfirst), put(pl.rowbase)};
+  }
+  std::vector<int32_t> prob_of_edge(E);
+  for (int e = 0; e < E; ++e) prob_of_edge[e] = c->cmp_prob[c->cmp_of_frame[c->h_edges[e].src]];
+  c->cmp_edge_map = put(prob_of_edge);
+  std::vector<size_t> fo(P + 1, 0);
+  for (int q = 0; q < P; ++q) { const size_t n = c->cmp_n[q]; fo[q + 1] = fo[q] + 2 * n * n + 6 * n + (size_t)plans[q].l_size; }
+  RET(c->d_cmp_i32.reserve(sizeof(int32_t) * blob.size()));
+  RET(c->d_cmp_f64.reserve(sizeof(double) * fo[P]));
+  RET(c->d_cmp_prob.reserve(sizeof(LmProblem) * P));
+  RET(c->d_cmp_state.reserve(sizeof(LmState) * (P + 1)));   // [P]: the whole graph, for lm_init_kernel
+  RET(c->d_cmp_ticket.reserve(sizeof(unsigned int)));
+  const int32_t* ib = c->d_cmp_i32.as<int32_t>();
+  std::vector<LmProblem> probs(P);
+  size_t dyn = 0;
+  for (int q = 0; q < P; ++q) {
+    const int n = c->cmp_n[q]; const Off& o = io[q];
+    LmProblem& p = probs[q];
+    std::memset(&p, 0, sizeof p);
+    p.S = c->d_cmp_state.as<LmState>() + q;
+    p.frame = ib + o.frame; p.edge = ib + o.edge;
+    NormalLayout& l = p.lay;
+    l.col = ib + o.col;
+    l.hb_ptr = ib + o.hb_ptr; l.hb_row = ib + o.hb_row; l.hb_col = ib + o.hb_col; l.hc_edge = ib + o.hc_edge; l.hc_sub = ib + o.hc_sub;
+    l.n_hblocks = (int32_t)plans[q].hb_row.size();
+    l.gb_ptr = ib + o.gb_ptr; l.gc_edge = ib + o.gc_edge; l.gc_side = ib + o.gc_side;
+    l.rlast = ib + o.rlast; l.rfirst = ib + o.rfirst; l.rowbase = ib + o.rowbase;
+    double* d = c->d_cmp_f64.as<double>() + fo[q];
+    p.H = d; d += (size_t)n * n; p.Hc = d; d += (size_t)n * n;
+    p.g = d; d += n; p.gc = d; d += n; p.scale = d; d += n; p.diag = d; d += n; p.step = d; d += n; l.rhs = d; d += n;
+    l.Lg = d;
+    // the factor stays in shared memory when it fits with its vectors (the bound of run_steps); else this component alone
+    // factors in global memory
+    const size_t vec = sizeof(double) * 3 * (size_t)(n + 1), lb = sizeof(double) * (size_t)plans[q].l_size;
+    l.l_in_smem = lb + vec <= 220 * 1024 ? 1 : 0;
+    dyn = std::max(dyn, vec + (l.l_in_smem ? lb : 0));
+  }
+  c->cmp_dyn = dyn;
+  CU(cudaMemcpyAsync(c->d_cmp_i32.p, blob.data(), sizeof(int32_t) * blob.size(), cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemcpyAsync(c->d_cmp_prob.p, probs.data(), sizeof(LmProblem) * P, cudaMemcpyHostToDevice, c->stream));
+  // the step kernel writes only the listed blocks of H and Hc; everything else stays zero from here
+  CU(cudaMemsetAsync(c->d_cmp_f64.p, 0, sizeof(double) * fo[P], c->stream));
+  CU(cudaMemsetAsync(c->d_cmp_ticket.p, 0, sizeof(unsigned int), c->stream));
+  CU(cudaStreamSynchronize(c->stream));   // the host vectors above must outlive their copies
+  c->cmp_key = key;
+  return MVICP_OK;
+}
+
+extern "C" {
+int mvicp_get_components(mvicp_ctx* c, int32_t* n_components, int32_t* component_of_frame) {
+  if (!c || !n_components) return fail(MVICP_ERR_INVALID, "mvicp_get_components: bad arguments");
+  if (!c->M) return fail(MVICP_ERR_STATE, "mvicp_get_components: frames must be set first");
+  std::vector<int32_t> comp;
+  *n_components = graph_components(c, comp);
+  if (component_of_frame) std::memcpy(component_of_frame, comp.data(), sizeof(int32_t) * c->M);
+  return MVICP_OK;
+}
+
+// Every component solved as mvicp_optimize solves it in a context that holds only that component: its lowest frame fixed, its
+// own trust region, counters and termination.  One pipelined loop for all of them: the streaming kernels skip the edges of the
+// components that are done, lm_step_components_kernel steps each of the others in its own CTA.
+int mvicp_optimize_components(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt_in,
+                              mvicp_lm_summary* summaries) {
+  if (!c || !c->M || !c->E) return fail(MVICP_ERR_STATE, "mvicp_optimize_components: frames and graph must be set first");
+  if (param < 0 || param > 2 || cost < 0 || cost > 2) return fail(MVICP_ERR_INVALID, "mvicp_optimize_components: bad param/cost");
+  if (cost != COST_P2P && !c->have_normals) return fail(MVICP_ERR_INVALID, "point-to-plane needs normals for every frame");
+  if (c->world > 1) return fail(MVICP_ERR_STATE, "mvicp_optimize_components: the component solve runs on one GPU; this context is sharded");
+  CU(cudaSetDevice(c->device));
+  const int M = c->M, E = c->E;
+  {   // the lowest frame of every component is fixed, as mvicp_optimize fixes frame 0 (icp-ceres.cpp:242-244)
+    std::vector<int32_t> comp;
+    std::vector<uint8_t> seen(graph_components(c, comp), 0);
+    for (int f = 0; f < M; ++f) if (!seen[comp[f]]) { seen[comp[f]] = 1; c->fixed[f] = 1; }
+  }
+  mvicp_lm_options opt; if (opt_in) opt = *opt_in; else mvicp_default_lm_options(&opt);
+  if (std::all_of(c->fixed.begin(), c->fixed.end(), [](uint8_t v) { return v != 0; })) {   // no component has anything to optimise
+    if (summaries) { int32_t K = 0; RET(mvicp_get_components(c, &K, nullptr)); for (int k = 0; k < K; ++k) summary_no_unknowns(summaries + k); }
+    return MVICP_OK;
+  }
+  RET(refresh_if_fixed_changed(c));
+  std::vector<uint8_t> key(c->fixed); key.push_back((uint8_t)(c->graph_gen & 0xff)); key.push_back((uint8_t)((c->graph_gen >> 8) & 0xff));
+  if (key != c->cmp_key) RET(build_component_layouts(c, key));
+  const int P = c->n_prob;
+  std::vector<LmState> st(P + 1);
+  std::memset(st.data(), 0, sizeof(LmState) * (P + 1));
+  for (int q = 0; q <= P; ++q) {
+    LmState& s = st[q];
+    s.opt = opt; s.param = param; s.cost_kind = cost; s.robust = robust ? 1 : 0; s.G = ambient_size(param);
+    if (q == P) { s.M = M; s.E = E; continue; }
+    s.M = c->cmp_M[q]; s.E = c->cmp_E[q]; s.n = c->cmp_n[q]; s.F = s.n / 6;
+    s.radius = opt.initial_trust_region_radius; s.decrease_factor = 2.0;
+  }
+  LmState* dS = c->d_cmp_state.as<LmState>();
+  CU(cudaMemcpyAsync(dS, st.data(), sizeof(LmState) * (P + 1), cudaMemcpyHostToDevice, c->stream));
+  // the per-frame arrays of the evaluation point are shared by every component (indexed by graph frame)
+  RET(c->d_x.reserve(sizeof(double) * 7 * M)); RET(c->d_cand.reserve(sizeof(double) * 7 * M));
+  RET(c->d_Rt.reserve(sizeof(Rt) * M)); RET(c->d_K.reserve(sizeof(double) * 36 * M));
+  RET(c->d_eout.reserve(sizeof(double) * EOUT * E));
+  c->nonrigid = poses_nonrigid(c->h_poses.data(), M);
+  const bool general = c->nonrigid && param != PARAM_AA;   // one eval path for the whole batch
+  if (general) { RET(c->d_gen.reserve(sizeof(FrameGen) * M)); RET(c->d_partial.reserve(sizeof(double) * GBLK * std::max<size_t>(1, c->n_eval_tiles))); }
+  LmWork w{};
+  w.S = dS + P; w.edges = c->d_edges.as<EdgeDev>(); w.eout = c->d_eout.as<double>(); w.world = 1;
+  w.x = c->d_x.as<double>(); w.cand = c->d_cand.as<double>(); w.Rt_eval = c->d_Rt.as<Rt>(); w.K_eval = c->d_K.as<double>();
+  w.G_eval = general ? c->d_gen.as<FrameGen>() : nullptr;
+  w.lay.poses16 = c->d_poses.as<double>(); w.lay.host_flag = c->d_flag;
+  const LmProblem* probs = c->d_cmp_prob.as<LmProblem>();
+  unsigned int* ticket = c->d_cmp_ticket.as<unsigned int>();
+
+  CU(cudaEventRecord(c->ev[3], c->stream));
+  lm_init_kernel<<<(M + 63) / 64, 64, 0, c->stream>>>(w);
+  c->stats.kernel_launches += 1;
+  const int max_evals = opt.max_num_iterations + 2;   // per component, so for the loop as well
+  const DoneGate gate{&dS[0].done, c->d_cmp_i32.as<int32_t>() + c->cmp_edge_map, (int32_t)(sizeof(LmState) / sizeof(int))};
+  auto eval = [&]() {
+    if (general) { if (c->f32) launch_eval_general<true>(c, param, cost, st[0].robust, gate); else launch_eval_general<false>(c, param, cost, st[0].robust, gate); }
+    else if (c->f32) launch_eval<true>(c, cost, st[0].robust, gate); else launch_eval<false>(c, cost, st[0].robust, gate);
+  };
+  auto step = [&](size_t) -> int {   // launched with the components' own shared-memory size (see run_steps below)
+    PeerTable pt; std::memset(&pt, 0, sizeof pt); pt.world = 1; pt.rank = 0;
+    if (general)
+      lm_edge_general_kernel<<<E, EDGE_THREADS, 0, c->stream>>>(c->d_edges.as<EdgeDev>(), c->d_edge_tile_begin.as<int32_t>(),
+                                                                c->d_partial.as<double>(), c->d_eout.as<double>(), gate, pt, 0, nullptr);
+    else
+      lm_edge_kernel<<<E, EDGE_THREADS, 0, c->stream>>>(c->d_edges.as<EdgeDev>(), c->d_edge_tile_begin.as<int32_t>(), c->d_partial.as<double>(),
+                                                        cost == COST_P2PLANE ? NBLK_PLANE : NBLK, c->d_Rt.as<Rt>(), c->d_K.as<double>(),
+                                                        c->d_eout.as<double>(), gate, pt, 0, nullptr);
+    lm_step_components_kernel<<<P, STEP_THREADS, c->cmp_dyn, c->stream>>>(w, probs, ticket);
+    c->stats.kernel_launches += (c->n_eval_tiles ? 1 : 0) + 2;
+    return MVICP_OK;
+  };
+  // run_steps drives the ring through w.lay.seq.  Its shared-memory sizing (from a whole graph's n and c->l_size, written to
+  // w.lay.l_in_smem and passed to `step`) does not apply here and is unused: every LmProblem carries its own l_in_smem, and
+  // `step` launches with c->cmp_dyn, the maximum over the components (the kernel attribute run_steps sets is the 220 KB bound).
+  RET(run_steps(c, lm_step_components_kernel, 0, max_evals, "LM (components)", w.lay, eval, step));
+  RET(read_back_solve(c, st.data(), dS, sizeof(LmState) * (P + 1)));
+  int max_iters = 0; bool all_done = true;
+  for (int q = 0; q < P; ++q) { max_iters = std::max(max_iters, (int)st[q].iteration); all_done = all_done && st[q].done; }
+  c->last_lm_iters = max_iters;   // the cross-round shortcuts of mvicp_correspond wait for the slowest component
+  if (summaries)
+    for (int k = 0; k < c->n_cmp; ++k) {
+      if (c->cmp_prob[k] < 0) summary_no_unknowns(summaries + k);
+      else summary_of_state(st[c->cmp_prob[k]], summaries + k);
+    }
+  if (st[P].nonrigid && !general)
+    return fail(MVICP_ERR_NONRIGID, "a pose's quaternion is not unit (non-rigid Isometry) but the unit-quaternion LM path was run");
+  if (!all_done) return fail(MVICP_ERR_STATE, "LM loop did not terminate within %d evaluations", max_evals);
   return MVICP_OK;
 }
 

@@ -5,7 +5,7 @@ usage: python tools/chol_host_check.py [--tsan]      (development aid; g++ >= 11
 import os, subprocess, sys, tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 src = open(os.path.join(ROOT, "mv_lm_icp_b200", "csrc", "lm_step.cuh")).read()
-fn = src[src.index("__device__ __forceinline__ void chol_factor_diag("):src.index("__global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel")]
+fn = src[src.index("__device__ __forceinline__ void chol_factor_diag("):src.index("// ---- the LM trust-region state machine")]
 harness = r'''
 #include <barrier>
 #include <thread>
