@@ -42,8 +42,10 @@ enum { MVICP_FLAG_NO_CERT = 128,         /* NN search: never keep a match on the
                                         CERT): every query of every round is searched */
        MVICP_FLAG_NO_SELECT_GUESS = 64, /* median select: always the three histogram passes, never the guess checked by the NN kernel's epilogue
                                         (csrc/select.cuh) in rounds that follow a one-iteration solve */
-       MVICP_FLAG_STEP_LOOP = 32, /* NN search: round 1's single loop of uniform steps instead of the while-while loop (csrc/knn.cuh
-                                      nn_drain); same matches, for A/B measurements */
+       MVICP_FLAG_STEP_LOOP = 32, /* NN search, rounds after the far ones: every query searched by its own lane (csrc/knn.cuh nn_search, the
+                                      single loop of uniform steps of nn_drain) instead of the warp's shared packet walk for the queries the
+                                      neighbour lists do not settle (nn_search_packet); no certificates, no guessed select; same matches, the
+                                      reference for tests and A/B measurements */
        MVICP_FLAG_NO_ADJ = 8,     /* NN search: do not use the per-leaf neighbour lists (csrc/adjacency.h) that let a seeded query inside its
                                       start leaf's reach skip the tree walk; same matches, for A/B measurements */
        MVICP_FLAG_HOST_BUILD = 4,  /* build the per-frame search trees on the host (csrc/tree_build.h) instead of on the device

@@ -159,15 +159,19 @@ __device__ __forceinline__ float pt_d32(const float4& r, const Q& s) {
 }
 
 // two points of a leaf per step (the point arrays are padded with +inf up to a multiple of LEAF)
+// track = false (certificates only): the screen values do not enter m1 / m2 -- the lane has scanned these points before, or is not
+// searching; a data select rather than a branch, so that a warp walking together stays converged
 template <bool F32, class Q>
-__device__ __forceinline__ void nn_leaf_step(const FrameDev& fd, int leaf, int sub, Q& s) {
+__device__ __forceinline__ void nn_leaf_step(const FrameDev& fd, int leaf, int sub, Q& s, bool track = true) {
   const int64_t pos = (int64_t)leaf * LEAF + 2 * sub;
   if (pos >= fd.n) return;   // padding leaf of the implicit tree (reachable only while the bound is still infinite)
   const float4 r0 = __ldg(fd.pts_sf + pos), r1 = __ldg(fd.pts_sf + pos + 1);
   const float d0 = pt_d32(r0, s), d1 = pt_d32(r1, s);
   if constexpr (nn_track<Q>::value) {
-    s.m2 = fminf(s.m2, fmaxf(s.m1, d0)); s.m1 = fminf(s.m1, d0);
-    s.m2 = fminf(s.m2, fmaxf(s.m1, d1)); s.m1 = fminf(s.m1, d1);
+    const float inf = __int_as_float(0x7f800000);
+    const float t0 = track ? d0 : inf, t1 = track ? d1 : inf;
+    s.m2 = fminf(s.m2, fmaxf(s.m1, t0)); s.m1 = fminf(s.m1, t0);
+    s.m2 = fminf(s.m2, fmaxf(s.m1, t1)); s.m1 = fminf(s.m1, t1);
     int before = s.bi;
     if (d0 <= s.bound32) { nn_exact<F32>(fd, pos, r0, s); if (s.bi != before) { s.v1 = d0; before = s.bi; } }
     if (d1 <= s.bound32) { nn_exact<F32>(fd, pos + 1, r1, s); if (s.bi != before) s.v1 = d1; }
@@ -328,6 +332,95 @@ __device__ __forceinline__ void nn_query_init(NNQuery& s, double qx, double qy, 
   s.bound32 = __int_as_float(0x7f800000);
 }
 
+// query transform, the operation sequence of knn_one (frame.cpp:117-118,131,136): g = R_s p + t_s ; q = Rinv_d (g - t_d)
+__device__ __forceinline__ void edge_query(const EdgeXf& sx, double px, double py, double pz, double& qx, double& qy, double& qz) {
+  const double gx = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(sx.Rs[0], px), __dmul_rn(sx.Rs[1], py)), __dmul_rn(sx.Rs[2], pz)), sx.ts[0]);
+  const double gy = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(sx.Rs[3], px), __dmul_rn(sx.Rs[4], py)), __dmul_rn(sx.Rs[5], pz)), sx.ts[1]);
+  const double gz = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(sx.Rs[6], px), __dmul_rn(sx.Rs[7], py)), __dmul_rn(sx.Rs[8], pz)), sx.ts[2]);
+  const double ex = __dsub_rn(gx, sx.td[0]), ey = __dsub_rn(gy, sx.td[1]), ez = __dsub_rn(gz, sx.td[2]);
+  qx = __dadd_rn(__dadd_rn(__dmul_rn(sx.Rinv[0], ex), __dmul_rn(sx.Rinv[1], ey)), __dmul_rn(sx.Rinv[2], ez));
+  qy = __dadd_rn(__dadd_rn(__dmul_rn(sx.Rinv[3], ex), __dmul_rn(sx.Rinv[4], ey)), __dmul_rn(sx.Rinv[5], ez));
+  qz = __dadd_rn(__dadd_rn(__dmul_rn(sx.Rinv[6], ex), __dmul_rn(sx.Rinv[7], ey)), __dmul_rn(sx.Rinv[8], ez));
+}
+
+// ---- packet walk: the 32 queries of a warp share one depth-first walk of the dst tree -----------------------------------------------
+// Each lane has run its own prologue (a start-leaf scan, the greedy descent) for a first bound.  Then at every step all lanes look
+// at the same node or leaf -- one broadcast load per warp.  A child is kept if any lane's bound admits it and the one with the
+// smaller lower bound (over those lanes) is visited first; a popped entry is skipped when its lower bound exceeds every lane's bound,
+// a popped leaf is first re-tested per lane.  Every node that can hold a point within a lane's bound is visited for that lane, and the
+// arg-min with the lowest-index tie rule does not depend on the order in which candidates are met: same results as nn_search, bit
+// for bit.  The stack holds at most one entry per level of the current path (<= depth < 32): entry i lives in a register of lane i.
+// live = false: the lane has no query or its prologue settled it; it votes with a bound that admits nothing and records nothing --
+//   only its bound32 is overwritten, its result and certificate terms stay as they are.
+// skip0, skip1: leaf nodes the lane's prologue already scanned (or -1).  The lane does not vote for them, and when the warp visits
+//   one anyway its screen values do not enter the lane's m1 / m2: a second scan would make the winner its own runner-up in the
+//   certificate (nn_margin).  (Every lane runs every leaf scan: a lane that is not live admits nothing, and a lane re-scanning its own
+//   points cannot change its best.  A lane-dependent branch around the scan left the warp unconverged at the pop, whose node index
+//   and stack pointer sm_90a code keeps in uniform registers -- DESIGN 4.1.)
+// Certificates (Q = NNQueryT): a live lane records its own lower bound for every child and every popped entry it does not visit
+//   (nn_pruned), except for its skipped leaves, whose points its m1 / m2 already hold; a leaf the warp visits is scanned by every live
+//   lane whose bound it exceeds as well, which only adds screen values of real points.
+// lb_of(node) is the fp32 lower bound of a node's box (axis-aligned in knn.cuh, hybrid oriented in far.cuh).
+template <bool F32, class Q, class LBF>
+__device__ __forceinline__ void nn_packet_walk(const FrameDev& fd, Q& s, bool live, int skip0, int skip1, LBF lb_of) {
+  const unsigned full = 0xffffffffu, inf_bits = 0x7f800000u;
+  const float inf = __uint_as_float(inf_bits);
+  const int L = fd.n_leaf_pad;
+  const int lane = threadIdx.x & 31;
+  if (!live) s.bound32 = -1.0f;
+  int my_n = 0; float my_lb = 0.f;   // stack entry `lane`
+  int sp = 0, node = 1;
+  while (true) {
+    if (node < L) {
+      const int c0 = 2 * node;
+      const float l0 = lb_of(c0), l1 = lb_of(c0 + 1);
+      const bool i0 = l0 <= s.bound32, i1 = l1 <= s.bound32;
+      const bool k0 = i0 && c0 != skip0 && c0 != skip1, k1 = i1 && c0 + 1 != skip0 && c0 + 1 != skip1;
+      if constexpr (nn_track<Q>::value) { nn_pruned(s, live && !i0 ? l0 : inf); nn_pruned(s, live && !i1 ? l1 : inf); }
+      const unsigned b0 = __ballot_sync(full, k0), b1 = __ballot_sync(full, k1);
+      if (b0 && b1) {
+        // non-negative floats order like their bit patterns: one integer min per child
+        const unsigned m0 = __reduce_min_sync(full, k0 ? __float_as_uint(l0) : inf_bits);
+        const unsigned m1 = __reduce_min_sync(full, k1 ? __float_as_uint(l1) : inf_bits);
+        const bool f0 = m0 <= m1;
+        if (lane == sp) { my_n = f0 ? c0 + 1 : c0; my_lb = __uint_as_float(f0 ? m1 : m0); }
+        ++sp;
+        node = f0 ? c0 : c0 + 1;
+        continue;
+      }
+      if (b0 | b1) { node = b0 ? c0 : c0 + 1; continue; }
+    } else {
+      const bool first = live && node != skip0 && node != skip1;
+#pragma unroll
+      for (int sub = 0; sub < LEAF / 2; ++sub) nn_leaf_step<F32, Q>(fd, node - L, sub, s, first);
+    }
+    node = -1;
+    while (sp > 0) {
+      --sp;
+      const int nd = __shfl_sync(full, my_n, sp);
+      const float m = __shfl_sync(full, my_lb, sp);
+      if (m > __uint_as_float(__reduce_max_sync(full, __float_as_uint(fmaxf(s.bound32, 0.f))))) {
+        if constexpr (nn_track<Q>::value) {   // beyond every lane's bound, so beyond this lane's (unless it skips the leaf)
+          const float l = lb_of(nd);
+          nn_pruned(s, live && !(l <= s.bound32) ? l : inf);
+        }
+        continue;
+      }
+      if (nd >= L) {
+        const float l = lb_of(nd);
+        const bool i = l <= s.bound32;
+        if (!__ballot_sync(full, i && nd != skip0 && nd != skip1)) {
+          if constexpr (nn_track<Q>::value) nn_pruned(s, live && !i ? l : inf);
+          continue;
+        }
+      }
+      node = nd;
+      break;
+    }
+    if (node < 0) break;
+  }
+}
+
 // One (edge, src point) query: transform, seed, [certificate test], search, results.  MODE 0: always search; 1: keep the match if
 // the certificate allows it (returns 1), otherwise do nothing and return 0 -- the caller searches it later; 2: search (no test).
 template <bool F32, bool WW, int CERT, int MODE>
@@ -376,6 +469,77 @@ __device__ __forceinline__ int knn_one(const FrameDev& fs, const FrameDev& fd, c
   return 1;
 }
 
+// Exact 1-NN for the 32 queries of a warp, every lane calls it (has = the lane holds a query, initialised in s).  Each lane runs
+// nn_search's prologue on its own: the start-leaf scan, the neighbour lists (nn_adj_fast), then the stale-seed rule or the greedy
+// descent.  A lane the neighbour lists settle is done; the others share one packet walk (nn_packet_walk) instead of each walking the
+// ancestors with a local-memory stack in a diverged warp, and a warp with no such lane skips the walk.  Same result as nn_search.
+template <bool F32, class Q>
+__device__ __forceinline__ void nn_search_packet(const FrameDev& fd, Q& s, bool has, int start_leaf) {
+  const int L = fd.n_leaf_pad;
+  int skip0 = -1, skip1 = -1;
+  bool live = has;
+  if (has) {
+    if (start_leaf >= 0) {
+      skip0 = L + start_leaf;
+#pragma unroll
+      for (int sub = 0; sub < LEAF / 2; ++sub) nn_leaf_step<F32, Q>(fd, start_leaf, sub, s);
+      const float4* b = reinterpret_cast<const float4*>(fd.boxes + skip0);
+      const float4 u = __ldg(b), v = __ldg(b + 1);
+      if (nn_adj_fast<F32, Q>(fd, s, start_leaf, u, v)) live = false;
+      else {   // the stale-seed rule of nn_search
+        const float bx = u.w - u.x, by = v.x - u.y, bz = v.y - u.z;
+        if (s.bound32 > 16.0f * fmaf(bz, bz, fmaf(by, by, bx * bx))) start_leaf = -1;
+      }
+    }
+    if (live && start_leaf < 0) {
+      int node = 1;
+      while (node < L) {
+        const int c0 = 2 * node;
+        const float l0 = box_lb32(fd.boxes, c0, s), l1 = box_lb32(fd.boxes, c0 + 1, s);
+        node = (l1 < l0) ? c0 + 1 : c0;
+      }
+      if (node != skip0) {
+#pragma unroll
+        for (int sub = 0; sub < LEAF / 2; ++sub) nn_leaf_step<F32, Q>(fd, node - L, sub, s);
+      }
+      skip1 = node;
+    }
+  }
+  if (__ballot_sync(0xffffffffu, live))
+    nn_packet_walk<F32, Q>(fd, s, live, skip0, skip1, [&](int nd) { return box_lb32(fd.boxes, nd, s); });
+}
+
+// knn_one (MODE 0) with the packet fall-through (nn_search_packet); every lane of the warp calls it (has = the lane holds a query)
+template <bool F32, int CERT>
+__device__ __forceinline__ void knn_one_packet(const FrameDev& fs, const FrameDev& fd, const EdgeXf& sx, const EdgeDev& e, int ks, bool has,
+                                               int32_t* corr, double* __restrict__ d2out, const int32_t* seed, double thresh,
+                                               float4* __restrict__ certs, bool& inlier, double& best) {
+  typedef typename std::conditional<CERT != 0, NNQueryT, NNQuery>::type QT;
+  QT nq;
+  int orig = 0, start_leaf = -1;
+  if (has) {
+    double px, py, pz, qx, qy, qz;
+    Rec<F32>::load(fs.pts_s, ks, px, py, pz, orig);
+    edge_query(sx, px, py, pz, qx, qy, qz);
+    nn_query_init(nq, qx, qy, qz, fd.absmax);
+    if constexpr (CERT != 0) nn_track_init(nq);
+    if (seed) {   // previous round's match: a valid first guess, the search stays exact
+      const int sd = seed[e.off + orig];
+      const int si = sd >= 0 ? sd : ~sd;
+      if (si >= 0 && si < fd.n) start_leaf = __ldg(fd.pos_of + si) / LEAF;
+    }
+  } else {
+    nn_query_init(nq, 0.0, 0.0, 0.0, fd.absmax);
+  }
+  nn_search_packet<F32, QT>(fd, nq, has, start_leaf);
+  if (!has) return;
+  if constexpr (CERT != 0) certs[e.off + ks] = make_float4(nq.fx, nq.fy, nq.fz, nn_margin(nq));
+  best = nq.best; const int bi = nq.bi;
+  inlier = best <= thresh;
+  corr[e.off + orig] = inlier ? bi : ~bi;
+  d2out[e.off + orig] = best;
+}
+
 // what a finished query contributes to the guessed median select; every lane of the warp calls it (`done` = has a result)
 __device__ __forceinline__ void knn_sel_account(const SelGuess& sg, int edge, int n_edges, bool done, bool inlier, double best, unsigned int* s_cnt) {
   const unsigned long long key = (unsigned long long)__double_as_longlong(best);
@@ -391,6 +555,8 @@ __device__ __forceinline__ void knn_sel_account(const SelGuess& sg, int edge, in
 
 // One thread per (edge, src point) query; src points are walked in the src frame's tree order so that the
 // lanes of a warp descend the dst tree together.
+// WW = true: the queries the neighbour lists do not settle share one packet walk per warp (knn_one_packet); WW = false
+// (MVICP_FLAG_STEP_LOOP): every lane runs nn_search with the one-step loop of nn_drain -- the per-lane reference.
 // SEL: the epilogue also feeds the guessed median select (select.cuh): per edge, the number of inliers, the number of inliers
 // below the guessed window of keys, and the keys inside the window.
 // CERT = 1 (needs seeds): every query also leaves a certificate {its position, the margin by which its match beats everything
@@ -414,10 +580,12 @@ knn_kernel(const FrameDev* __restrict__ frames, const EdgeDev* __restrict__ edge
   const FrameDev fs = frames[e.src];
   const FrameDev fd = frames[e.dst];
   const int ks = t.start + threadIdx.x;
-  if (!SEL && ks >= e.n_src) return;
+  // the packet walk needs the whole warp: only a warp wholly past the edge's end leaves early
+  if (!SEL && (WW ? t.start + (int)(threadIdx.x & ~31u) : ks) >= e.n_src) return;
   bool inlier = false; double best = 0.0;
   const bool has = ks < e.n_src;
-  if (has) knn_one<F32, WW, CERT, 0>(fs, fd, sx, e, ks, corr, d2out, seed, thresh, certs, inlier, best);
+  if (WW) knn_one_packet<F32, CERT>(fs, fd, sx, e, ks, has, corr, d2out, seed, thresh, certs, inlier, best);
+  else if (has) knn_one<F32, false, CERT, 0>(fs, fd, sx, e, ks, corr, d2out, seed, thresh, certs, inlier, best);
   if (SEL) {   // every thread of the CTA arrives here
     knn_sel_account(sg, t.edge, n_edges, has, inlier, best, s_cnt);
     __syncthreads();

@@ -42,6 +42,11 @@ static inline void __syncthreads() {}
 // declarations only, so that the kernels' text parses: the host check calls the search functions, never a kernel
 unsigned __ballot_sync(unsigned, int);
 unsigned __match_any_sync(unsigned, int);
+unsigned __reduce_min_sync(unsigned, unsigned);
+unsigned __reduce_max_sync(unsigned, unsigned);
+template <class T> T __shfl_sync(unsigned, T, int, int = 32);
+static inline unsigned __float_as_uint(float f) { unsigned i; std::memcpy(&i, &f, 4); return i; }
+static inline float __uint_as_float(unsigned i) { float f; std::memcpy(&f, &i, 4); return f; }
 static inline int __popc(unsigned x) { return __builtin_popcount(x); }
 template <class T> T atomicAdd(T*, T);
 static inline void __syncwarp() {}
