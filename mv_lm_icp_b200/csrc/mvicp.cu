@@ -376,6 +376,31 @@ void mvicp_default_lm_options(mvicp_lm_options* o) {
   o->function_tolerance = 1e-6; o->gradient_tolerance = 1e-10; o->parameter_tolerance = 1e-8;
 }
 
+}  // extern "C"
+// The rules of mvicp_lm_options (include/mvicp.h): what Ceres' Solver::Options::IsValid rejects for a trust-region LM solve.
+// Every test is written as "the valid case holds", so a NaN fails it.  Called before an entry point changes any state; a null
+// pointer stands for the defaults.
+static int check_lm_options(const mvicp_lm_options* o, const char* fn) {
+  if (!o) return MVICP_OK;
+  const char* bad = nullptr;
+  if (!(o->max_num_iterations >= 0)) bad = "max_num_iterations < 0";
+  else if (!(o->max_num_consecutive_invalid_steps >= 0)) bad = "max_num_consecutive_invalid_steps < 0";
+  else if (!(o->function_tolerance >= 0.0)) bad = "function_tolerance < 0";
+  else if (!(o->gradient_tolerance >= 0.0)) bad = "gradient_tolerance < 0";
+  else if (!(o->parameter_tolerance >= 0.0)) bad = "parameter_tolerance < 0";
+  else if (!(o->initial_trust_region_radius > 0.0)) bad = "initial_trust_region_radius <= 0";
+  else if (!(o->max_trust_region_radius > 0.0)) bad = "max_trust_region_radius <= 0";
+  else if (!(o->min_trust_region_radius > 0.0)) bad = "min_trust_region_radius <= 0";
+  else if (!(o->min_trust_region_radius <= o->initial_trust_region_radius)) bad = "min_trust_region_radius > initial_trust_region_radius";
+  else if (!(o->initial_trust_region_radius <= o->max_trust_region_radius)) bad = "initial_trust_region_radius > max_trust_region_radius";
+  else if (!(o->min_relative_decrease >= 0.0)) bad = "min_relative_decrease < 0";
+  else if (!(o->min_lm_diagonal >= 0.0)) bad = "min_lm_diagonal < 0";
+  else if (!(o->max_lm_diagonal >= 0.0)) bad = "max_lm_diagonal < 0";
+  else if (!(o->min_lm_diagonal <= o->max_lm_diagonal)) bad = "min_lm_diagonal > max_lm_diagonal";
+  return bad ? fail(MVICP_ERR_INVALID, "%s: invalid LM options: %s (or NaN)", fn, bad) : MVICP_OK;
+}
+extern "C" {
+
 int mvicp_create(const mvicp_config* cfg, mvicp_ctx** out) {
   if (!out) return fail(MVICP_ERR_INVALID, "mvicp_create: out is null");
   int ndev = 0;
@@ -1286,6 +1311,7 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
   if (!c || !c->M || !c->E) return fail(MVICP_ERR_STATE, "mvicp_optimize: frames and graph must be set first");
   if (param < 0 || param > 2 || cost < 0 || cost > 2) return fail(MVICP_ERR_INVALID, "mvicp_optimize: bad param/cost");
   if (cost != COST_P2P && !c->have_normals) return fail(MVICP_ERR_INVALID, "point-to-plane needs normals for every frame");
+  RET(check_lm_options(opt_in, "mvicp_optimize"));
   CU(cudaSetDevice(c->device));
   const int M = c->M, E = c->E;
   c->fixed[0] = 1;   // frames[0]->fixed = true (icp-ceres.cpp:242-244,342-344,417-419)
@@ -1334,7 +1360,7 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
   CU(cudaEventRecord(c->ev[3], c->stream));
   lm_init_kernel<<<(M + 63) / 64, 64, 0, c->stream>>>(w);
   c->stats.kernel_launches += 1;
-  const int max_evals = opt.max_num_iterations + 2;
+  const int64_t max_evals = (int64_t)opt.max_num_iterations + 2;   // (no int overflow at INT32_MAX iterations)
   const bool use_p2p = c->comm && c->world > 1 && c->p2p_ok && E <= mvicp_ctx::X_ECAP;
   const DoneGate done_flag{&w.S->done, nullptr, 0};
   auto eval = [&]() {
@@ -1399,7 +1425,7 @@ int mvicp_optimize(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, co
   if (st.nonrigid == 2) return fail(MVICP_ERR_NCCL, "a peer rank never delivered its pair matrices (peer-memory exchange timed out)");
   if (st.nonrigid && !general)   // cannot happen after mvicp_set_poses; guards poses that reached the device another way
     return fail(MVICP_ERR_NONRIGID, "a pose's quaternion is not unit (non-rigid Isometry) but the unit-quaternion LM path was run");
-  if (!st.done) return fail(MVICP_ERR_STATE, "LM loop did not terminate within %d evaluations", max_evals);
+  if (!st.done) return fail(MVICP_ERR_STATE, "LM loop did not terminate within %lld evaluations", (long long)max_evals);
   return MVICP_OK;
 }
 
@@ -1521,6 +1547,7 @@ int mvicp_optimize_components(mvicp_ctx* c, int32_t param, int32_t cost, int32_t
   if (param < 0 || param > 2 || cost < 0 || cost > 2) return fail(MVICP_ERR_INVALID, "mvicp_optimize_components: bad param/cost");
   if (cost != COST_P2P && !c->have_normals) return fail(MVICP_ERR_INVALID, "point-to-plane needs normals for every frame");
   if (c->world > 1) return fail(MVICP_ERR_STATE, "mvicp_optimize_components: the component solve runs on one GPU; this context is sharded");
+  RET(check_lm_options(opt_in, "mvicp_optimize_components"));
   CU(cudaSetDevice(c->device));
   const int M = c->M, E = c->E;
   {   // the lowest frame of every component is fixed, as mvicp_optimize fixes frame 0 (icp-ceres.cpp:242-244)
@@ -1566,7 +1593,7 @@ int mvicp_optimize_components(mvicp_ctx* c, int32_t param, int32_t cost, int32_t
   CU(cudaEventRecord(c->ev[3], c->stream));
   lm_init_kernel<<<(M + 63) / 64, 64, 0, c->stream>>>(w);
   c->stats.kernel_launches += 1;
-  const int max_evals = opt.max_num_iterations + 2;   // per component, so for the loop as well
+  const int64_t max_evals = (int64_t)opt.max_num_iterations + 2;   // per component, so for the loop as well
   const DoneGate gate{&dS[0].done, c->d_cmp_i32.as<int32_t>() + c->cmp_edge_map, (int32_t)(sizeof(LmState) / sizeof(int))};
   auto eval = [&]() {
     if (general) { if (c->f32) launch_eval_general<true>(c, param, cost, st[0].robust, gate); else launch_eval_general<false>(c, param, cost, st[0].robust, gate); }
@@ -1600,11 +1627,12 @@ int mvicp_optimize_components(mvicp_ctx* c, int32_t param, int32_t cost, int32_t
     }
   if (st[P].nonrigid && !general)
     return fail(MVICP_ERR_NONRIGID, "a pose's quaternion is not unit (non-rigid Isometry) but the unit-quaternion LM path was run");
-  if (!all_done) return fail(MVICP_ERR_STATE, "LM loop did not terminate within %d evaluations", max_evals);
+  if (!all_done) return fail(MVICP_ERR_STATE, "LM loop did not terminate within %lld evaluations", (long long)max_evals);
   return MVICP_OK;
 }
 
 int mvicp_icp_round(mvicp_ctx* c, float thresh, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt, mvicp_lm_summary* summary) {
+  RET(check_lm_options(opt, "mvicp_icp_round"));   // before the correspondence step changes anything
   RET(mvicp_correspond(c, thresh));
   return mvicp_optimize(c, param, cost, robust, opt, summary);
 }
@@ -1613,6 +1641,7 @@ int mvicp_pairwise(const mvicp_config* cfg, int32_t param, int32_t cost, const d
                    int64_t n, const mvicp_lm_options* opt, double* pose16_out, mvicp_lm_summary* summary) {
   if (!src || !dst || n <= 0 || !pose16_out) return fail(MVICP_ERR_INVALID, "mvicp_pairwise: bad arguments");
   if (cost != MVICP_COST_P2P && !nor) return fail(MVICP_ERR_INVALID, "mvicp_pairwise: point-to-plane needs dst normals");
+  RET(check_lm_options(opt, "mvicp_pairwise"));
   return run_pairwise(cfg, src, dst, nor, n, pose16_out, [&](mvicp_ctx* c) { return mvicp_optimize(c, param, cost, 0, opt, summary); });
 }
 
