@@ -217,12 +217,15 @@ struct G2oWork {
   double *H, *g;                 // g = sum J^T Omega e: g2o's b is -g
   double* chi_calls;             // [max_calls + 1]: chi2 before the first call, then after every call
   double* trace;                 // [trace_cap][5]: lambda, chi, tchi, rho, accepted -- one row per trial
+  double* poses16;               // [M][16]
+  volatile int32_t* host_flag;   // mapped pinned ring: (sequence << 1) | done, written at the end of every step
+  int32_t seq;
 };
 
 __global__ void g2o_init_kernel(G2oWork w, int M) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= M) return;
-  Rt a; pose16_to_Rt(w.lay.poses16 + 16 * f, &a);
+  Rt a; pose16_to_Rt(w.poses16 + 16 * f, &a);
   w.x[f] = a; w.ev[f] = a; w.n_oplus[f] = 0;
 }
 
@@ -259,7 +262,7 @@ __global__ void __launch_bounds__(STEP_THREADS) g2o_step_kernel(G2oWork w) {
   __shared__ double red[40];
   __shared__ G2oState s_state;
   __shared__ int s_solve, s_accept, s_tobuild;
-  if (w.S->done) { if (threadIdx.x == 0) publish_step(w.lay, true); return; }
+  if (w.S->done) { if (threadIdx.x == 0) publish_step(w.host_flag, w.seq, true); return; }
   const int tid = threadIdx.x, T = blockDim.x;
   copy_state(&s_state, w.S);
   G2oState* S = &s_state;
@@ -372,10 +375,10 @@ __global__ void __launch_bounds__(STEP_THREADS) g2o_step_kernel(G2oWork w) {
   }
   if (s_tobuild && !S->done) for (int f = tid; f < M; f += T) w.ev[f] = w.x[f];
   if (S->done)   // write the vertices of the problem back; every other frame keeps its pose bit for bit
-    for (int f = tid; f < M; f += T) if (lay.col[f] >= 0) Rt_to_pose16(&w.x[f], lay.poses16 + 16 * f);
+    for (int f = tid; f < M; f += T) if (lay.col[f] >= 0) Rt_to_pose16(&w.x[f], w.poses16 + 16 * f);
   __syncthreads();
   copy_state(w.S, &s_state);
-  if (tid == 0) publish_step(lay, S->done);
+  if (tid == 0) publish_step(w.host_flag, w.seq, S->done);
 }
 
 }  // namespace mv

@@ -26,8 +26,8 @@ struct LmState {
   double radius, decrease_factor, x_cost, cand_cost, x_norm, initial_cost, model_cost_change, step_norm, gmax;
 };
 
-// The normal equations as both step kernels (lm_step_kernel, g2o_step_kernel) lay them out, gather them and report to the
-// host.  Built on the host from the free frames' local columns (mvicp.cu, build_normal_layout).
+// The normal equations as both step kernels (lm_step_kernel, g2o_step_kernel) lay them out and gather them.  Built on the host
+// from the free frames' local columns (mvicp.cu, upload_problems).
 struct NormalLayout {
   const int32_t* col;        // [M] first local column or -1
   // block-sparse gather lists (host-built, deterministic order)
@@ -37,9 +37,6 @@ struct NormalLayout {
   const int32_t* rowbase;                        // skyline storage of the factor: entry (r, c) at Lg[rowbase[r] + c]; [n] = rhs row
   double *Lg, *rhs;
   int32_t l_in_smem;
-  double* poses16;
-  volatile int32_t* host_flag; // mapped pinned ring: (sequence << 1) | done, written at the end of every step
-  int32_t seq;
 };
 
 struct LmWork {
@@ -53,20 +50,20 @@ struct LmWork {
   Rt* Rt_eval;               // [M]
   double* K_eval;            // [M][36]
   FrameGen* G_eval;          // [M] general frame model (null unless a quaternion is not unit)
-  NormalLayout lay;
-  double *H, *g, *Hc, *gc, *scale, *diag, *step;
+  double* poses16;           // [M][16]
+  volatile int32_t* host_flag; // mapped pinned ring: (sequence << 1) | done, written at the end of every step
+  int32_t seq;
   long long* prof;           // development aid (MVICP_STEP_PROFILE=1): clock64() stamps of the last solving launch, else null
 };
 
-// One LM problem as the state machine sees it: the whole graph (lm_step_kernel: frame and edge null, the layout and the dense
-// arrays of LmWork), or one connected component (lm_step_components_kernel).  Local frame f is frame frame[f] of the graph
-// (ascending), local edge e is edge edge[e] (graph order); the layout's columns, col[] and gb_ptr[] are over local frames, its
-// gather lists name graph edges.  x, cand, Rt_eval, K_eval, G_eval and the poses stay indexed by graph frame.
+// One LM problem as the state machine sees it: the whole graph, or one connected component.  Local frame f is frame frame[f] of
+// the graph (ascending), local edge e is edge edge[e] (graph order); the layout's columns, col[] and gb_ptr[] are over local
+// frames, its gather lists name graph edges.  x, cand, Rt_eval, K_eval, G_eval and the poses stay indexed by graph frame.
 struct LmProblem {
   LmState* S;
   const int32_t* frame;      // [S->M]
   const int32_t* edge;       // [S->E]
-  NormalLayout lay;          // (poses16, host_flag and seq are LmWork's)
+  NormalLayout lay;
   double *H, *g, *Hc, *gc, *scale, *diag, *step;
 };
 
@@ -125,16 +122,16 @@ __device__ __forceinline__ double edge_cost_sum(const double* eout, int E, doubl
   return block_sum(s, red);
 }
 // A step kernel works on a shared-memory copy of its state (dozens of dependent scalar reads per step) and writes it back once
-// at the end; nobody else touches the state while the kernel runs (lm_step_components_kernel stages its LmProblem the same way)
+// at the end; nobody else touches the state while the kernel runs (lm_step_kernel stages its LmProblem the same way)
 template <typename State> __device__ __forceinline__ void copy_state(State* dst, const State* src) {
   for (int i = threadIdx.x; i < (int)(sizeof(State) / sizeof(int32_t)); i += blockDim.x)
     reinterpret_cast<int32_t*>(dst)[i] = reinterpret_cast<const int32_t*>(src)[i];
   __syncthreads();
 }
 // One thread tells the host that this step ran: (sequence << 1) | done into the mapped ring, after every write of the step
-__device__ __forceinline__ void publish_step(const NormalLayout& l, bool done) {
+__device__ __forceinline__ void publish_step(volatile int32_t* host_flag, int32_t seq, bool done) {
   __threadfence();
-  l.host_flag[l.seq & 7] = (l.seq << 1) | (done ? 1 : 0);
+  host_flag[seq & 7] = (seq << 1) | (done ? 1 : 0);
   __threadfence_system();
 }
 
@@ -144,7 +141,7 @@ __global__ void lm_init_kernel(LmWork w) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= S->M) return;
   double x[7] = {0, 0, 0, 0, 0, 0, 0};
-  param_of_pose(S->param, w.lay.poses16 + 16 * f, x);
+  param_of_pose(S->param, w.poses16 + 16 * f, x);
   if (S->param != PARAM_AA) {
     const double n2 = x[0] * x[0] + x[1] * x[1] + x[2] * x[2] + x[3] * x[3];
     if (!(fabs(n2 - 1.0) <= 1e-9)) atomicExch(&S->nonrigid, 1);
@@ -321,23 +318,20 @@ __device__ bool chol_solve(double* L, const int32_t* __restrict__ rowbase, int n
 }
 
 // ---- the LM trust-region state machine: one step of one problem, one CTA -----------------------------------------------
-// COMP = false: the whole graph, which publishes the step into the ring itself; COMP = true: one connected component, whose
-// kernel publishes once every component's CTA has stepped.  Every loop over frames, edges and columns runs over the problem's
-// LOCAL indices, so a component's reductions are associated exactly as in a context that holds only that component.
-template <bool COMP>
+// Every loop over frames, edges and columns runs over the problem's LOCAL indices, so a component's reductions are associated
+// exactly as in a context that holds only that component.
 __device__ __forceinline__ void lm_step_body(const LmWork& w, const LmProblem& p) {
   extern __shared__ double smem[];
   __shared__ double red[40];
   __shared__ int s_flag;
-  if (p.S->done) { if (!COMP && threadIdx.x == 0) publish_step(w.lay, true); return; }
+  if (p.S->done) return;
   const int tid = threadIdx.x, T = blockDim.x;
   __shared__ LmState s_state;
   copy_state(&s_state, p.S);
   LmState* S = &s_state;
   const int n = S->n, M = S->M, E = S->E, param = S->param;
   const NormalLayout& lay = p.lay;
-  auto gf = [&](int f) { return COMP ? p.frame[f] : f; };   // local frame -> frame of the graph
-  long long* prof = w.prof ? w.prof + 16 * (w.lay.seq & 3) : nullptr;   // one row of stamps per launch, the last four launches kept
+  long long* prof = w.prof ? w.prof + 16 * (w.seq & 3) : nullptr;   // one row of stamps per launch, the last four launches kept
 #define MV_STAMP(i) do { if (prof && tid == 0) prof[i] = clock64(); } while (0)
   MV_STAMP(0);
   if (w.peer_flags) {   // wait until every rank's edge kernel has delivered this iteration's pair matrices
@@ -357,7 +351,7 @@ __device__ __forceinline__ void lm_step_body(const LmWork& w, const LmProblem& p
   gather_blocks(lay, w.eout, n, p.Hc);
   gather_gradient(lay, w.eout, M, p.gc);
   __syncthreads();
-  const double eval_cost = edge_cost_sum(w.eout, E, red, COMP ? p.edge : nullptr);
+  const double eval_cost = edge_cost_sum(w.eout, E, red, p.edge);
 
   MV_STAMP(1);
   // ================= 2. accept / reject / terminate =================================================
@@ -403,7 +397,7 @@ __device__ __forceinline__ void lm_step_body(const LmWork& w, const LmProblem& p
       p.H[at] = p.Hc[at];
     }
     for (int idx = tid; idx < n; idx += T) p.g[idx] = p.gc[idx];
-    for (int idx = tid; idx < M * 7; idx += T) { const int at = COMP ? 7 * gf(idx / 7) + idx % 7 : idx; w.x[at] = w.cand[at]; }
+    for (int idx = tid; idx < M * 7; idx += T) { const int at = 7 * p.frame[idx / 7] + idx % 7; w.x[at] = w.cand[at]; }
     __syncthreads();
     if (S->phase == 0)
       for (int j = tid; j < n; j += T) p.scale[j] = S->opt.jacobi_scaling ? 1.0 / (1.0 + sqrt(p.H[(size_t)j * n + j])) : 1.0;
@@ -413,7 +407,7 @@ __device__ __forceinline__ void lm_step_body(const LmWork& w, const LmProblem& p
       if (lay.col[f] < 0) continue;
       const int G = S->G;
       double xf[7], ng[6], xp[7];
-      for (int i = 0; i < G; ++i) { xf[i] = w.x[7 * gf(f) + i]; xs += xf[i] * xf[i]; }
+      for (int i = 0; i < G; ++i) { xf[i] = w.x[7 * p.frame[f] + i]; xs += xf[i] * xf[i]; }
       for (int i = 0; i < 6; ++i) ng[i] = -p.g[lay.col[f] + i];
       param_plus(param, xf, ng, xp);
       for (int i = 0; i < G; ++i) gm = fmax(gm, fabs(xf[i] - xp[i]));
@@ -493,7 +487,7 @@ __device__ __forceinline__ void lm_step_body(const LmWork& w, const LmProblem& p
     // candidate = Plus(x, step * scale) per free frame; step norm in the ambient space
     double sn = 0.0;
     for (int f = tid; f < M; f += T) {
-      const int G = S->G, g_f = gf(f);
+      const int G = S->G, g_f = __ldg(p.frame + f);   // (read-only path: 196 instead of 216 bytes of spills, ptxas 12.9)
       double xf[7], d[6], xp[7] = {0, 0, 0, 0, 0, 0, 0};
       for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * g_f + i];
       if (lay.col[f] >= 0) {
@@ -518,40 +512,41 @@ __device__ __forceinline__ void lm_step_body(const LmWork& w, const LmProblem& p
   // ================= 4. on termination: write every frame's pose back (icp-ceres.cpp:318-322,392-394,472-474)
   if (S->done) {
     for (int f = tid; f < M; f += T) {
-      double xf[7]; for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * gf(f) + i];
-      pose_of_param(param, xf, w.lay.poses16 + 16 * gf(f));
+      double xf[7]; for (int i = 0; i < 7; ++i) xf[i] = w.x[7 * p.frame[f] + i];
+      pose_of_param(param, xf, w.poses16 + 16 * p.frame[f]);
     }
   }
   __syncthreads();
   copy_state(p.S, &s_state);
   MV_STAMP(6);
-  if (!COMP && tid == 0) publish_step(w.lay, S->done);
-  MV_STAMP(7);
 #undef MV_STAMP
 }
 
-__global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w) {
-  const LmProblem p{w.S, nullptr, nullptr, w.lay, w.H, w.g, w.Hc, w.gc, w.scale, w.diag, w.step};
-  lm_step_body<false>(w, p);
-}
-
-// One CTA per connected component (probs[blockIdx.x]), each stepping its own problem.  Every CTA takes a ticket when its step is
-// written; the last one publishes (sequence << 1) | (every component done) into the ring and resets the ticket for the next
-// launch.  The problem's view is staged in shared memory once per CTA, not copied into every thread.
-__global__ void __launch_bounds__(STEP_THREADS) lm_step_components_kernel(LmWork w, const LmProblem* __restrict__ probs, unsigned int* ticket) {
+// One CTA per LM problem (probs[blockIdx.x]), each stepping its own problem.  Every CTA takes a ticket when its step is written;
+// the last one publishes (sequence << 1) | (every problem done) into the ring and resets the ticket for the next launch (a
+// single CTA publishes directly).  The problem's view is staged in shared memory once per CTA, not copied into every thread.
+__global__ void __launch_bounds__(STEP_THREADS) lm_step_kernel(LmWork w, const LmProblem* __restrict__ probs, unsigned int* ticket) {
   __shared__ LmProblem s_prob;
   copy_state(&s_prob, probs + blockIdx.x);
-  lm_step_body<true>(w, s_prob);
+  lm_step_body(w, s_prob);
   __shared__ int s_last;
   __syncthreads();
-  if (threadIdx.x == 0) { __threadfence(); s_last = atomicAdd(ticket, 1u) == gridDim.x - 1; }
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  int open = 0;
-  for (int k = threadIdx.x; k < (int)gridDim.x; k += blockDim.x) open |= *(volatile const int*)&probs[k].S->done == 0;
-  open = __syncthreads_count(open);
-  if (threadIdx.x == 0) { *ticket = 0u; publish_step(w.lay, open == 0); }
+  int open;
+  if (gridDim.x == 1) {   // one problem: no ticket (its atomic and fences cost ~2 us per step on an H100)
+    open = *(volatile const int*)&s_prob.S->done == 0;
+  } else {
+    if (threadIdx.x == 0) { __threadfence(); s_last = atomicAdd(ticket, 1u) == gridDim.x - 1; }
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    open = 0;
+    for (int k = threadIdx.x; k < (int)gridDim.x; k += blockDim.x) open |= *(volatile const int*)&probs[k].S->done == 0;
+    open = __syncthreads_count(open);
+  }
+  if (threadIdx.x == 0) {
+    *ticket = 0u; publish_step(w.host_flag, w.seq, open == 0);
+    if (w.prof) w.prof[16 * (w.seq & 3) + 7] = clock64();
+  }
 }
 
 }  // namespace mv

@@ -59,13 +59,11 @@ struct EdgeXf { double Rs[9], ts[3], Rinv[9], td[3]; };
 
 struct Tile { int32_t edge; int32_t start; };   // work item: `count` slots of one edge from `start`
 
-// Which evaluations of the pipelined LM loop have nothing left to do, because the solve that reads them terminated.  One
-// problem (comp null): its flag done[0].  One problem per connected component: edge e belongs to problem comp[e] (-1: to none,
-// all of its frames are fixed), whose flag is done[stride * comp[e]].
+// Which evaluations of the pipelined LM loop have nothing left to do, because the solve that reads them terminated: edge e
+// belongs to LM problem comp[e] (-1: to none, all of its frames are fixed), whose flag is done[stride * comp[e]].
 struct DoneGate {
   const int* done; const int32_t* comp; int32_t stride;
   __device__ __forceinline__ bool skip(int e) const {
-    if (!comp) return *done != 0;
     const int k = comp[e];
     return k < 0 || done[(size_t)stride * k] != 0;
   }

@@ -1,4 +1,5 @@
-"""Development aid: per-phase clock64() cycles of lm_step_kernel's launches (MVICP_STEP_PROFILE=1).  usage (GPU box):
+"""Development aid: per-phase clock64() cycles of lm_step_kernel's launches in a one-problem solve (MVICP_STEP_PROFILE=1; the
+joint optimize, or a component solve with one free component).  usage (GPU box):
 MVICP_STEP_PROFILE=1 python tools/step_profile.py [views] [points]
 With max_num_iterations = 1 a solve is two launches: #1 takes the initial evaluation, builds and factors the system and makes the
 candidate; #2 takes the candidate's evaluation, accepts or rejects it and stops."""
