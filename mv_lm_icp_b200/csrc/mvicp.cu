@@ -120,6 +120,8 @@ struct mvicp_ctx {
   std::vector<float> h_weight; std::vector<unsigned long long> h_count;
   // LM
   DevBuf d_x, d_cand, d_Rt, d_K, d_eout, d_posegather, d_gen;
+  int lm_blocks_E = 0;         // edges of the LM evaluation d_eout holds; 0: none since the graph was set, or a g2o solve reused it
+  std::vector<uint8_t> lm_blocks_fixed;   // the fixed flags of that solve: the edges of a fixed src read as zeros
   std::vector<int32_t> h_col;
   volatile int32_t* h_flag = nullptr; volatile int32_t* d_flag = nullptr;   // mapped pinned ring written by the step kernels
   uint32_t graph_gen = 0;
@@ -225,7 +227,7 @@ static int finish_set_frames(mvicp_ctx* c, int M) {
   for (int f = 0; f < M; ++f) for (int i = 0; i < 4; ++i) c->h_poses[16 * f + 5 * i] = 1.0;
   CU(cudaMemcpy(c->d_poses.p, c->h_poses.data(), sizeof(double) * 16 * M, cudaMemcpyHostToDevice));
   c->fixed.assign(M, 0); c->fixed[0] = 1;
-  c->E = 0; c->h_edges.clear(); c->have_corr = false;
+  c->E = 0; c->h_edges.clear(); c->have_corr = false; c->lm_blocks_E = 0;
   c->last_lm_iters = 1 << 20;
   return MVICP_OK;
 }
@@ -704,7 +706,7 @@ int mvicp_set_graph(mvicp_ctx* c, int32_t E, const int32_t* src, const int32_t* 
   for (int e = 0; e < E; ++e)
     if (src[e] < 0 || src[e] >= c->M || dst[e] < 0 || dst[e] >= c->M || src[e] == dst[e])
       return fail(MVICP_ERR_INVALID, "edge %d: (%d -> %d) invalid", e, src[e], dst[e]);
-  c->E = E; c->h_edges.assign(E, EdgeDev{});
+  c->E = E; c->h_edges.assign(E, EdgeDev{}); c->lm_blocks_E = 0;
   for (int e = 0; e < E; ++e) { c->h_edges[e].src = src[e]; c->h_edges[e].dst = dst[e]; }
   return rebuild_work(c);
 }
@@ -1364,6 +1366,7 @@ static int solve_lm(mvicp_ctx* c, bool per_component, const char* fn, int32_t pa
   if (per_component && c->world > 1) return fail(MVICP_ERR_STATE, "%s: the component solve runs on one GPU; this context is sharded", fn);
   RET(check_lm_options(opt_in, fn));
   CU(cudaSetDevice(c->device));
+  c->lm_blocks_E = 0;   // until this solve's evaluations have run
   const int M = c->M, E = c->E;
   std::vector<int32_t> comp(M, 0);
   const int K = per_component ? graph_components(c, comp) : 1;
@@ -1501,6 +1504,7 @@ static int solve_lm(mvicp_ctx* c, bool per_component, const char* fn, int32_t pa
   if (st[P].nonrigid && !general)   // cannot happen after mvicp_set_poses; guards poses that reached the device another way
     return fail(MVICP_ERR_NONRIGID, "a pose's quaternion is not unit (non-rigid Isometry) but the unit-quaternion LM path was run");
   if (!all_done) return fail(MVICP_ERR_STATE, "LM loop did not terminate within %lld evaluations", (long long)max_evals);
+  c->lm_blocks_E = E; c->lm_blocks_fixed = c->fixed;
   return MVICP_OK;
 }
 
@@ -1564,6 +1568,7 @@ int mvicp_optimize_g2o(mvicp_ctx* c, int32_t cost, const mvicp_g2o_options* opt_
   mvicp_g2o_options opt; if (opt_in) opt = *opt_in; else mvicp_default_g2o_options(&opt);
   if (opt.iterations_per_call < 1 || opt.max_calls < 1 || opt.max_trials < 1 || opt.no_improvement_limit < 0 || opt.orthonormalize_after < 0)
     return fail(MVICP_ERR_INVALID, "mvicp_optimize_g2o: bad options");
+  c->lm_blocks_E = 0;   // the g2o solve writes its own edge blocks into d_eout
   CU(cudaSetDevice(c->device));
   const int M = c->M, E = c->E;
   c->fixed[0] = 1;   // frames[0]->fixed = true (icp-g2o.cpp:182-186)
@@ -1974,6 +1979,34 @@ int mvicp_debug_step_profile(mvicp_ctx* c, long long* out64) {
   if (!c || !out64 || !c->d_prof.p) return fail(MVICP_ERR_STATE, "mvicp_debug_step_profile: run with MVICP_STEP_PROFILE=1");
   CU(cudaSetDevice(c->device));
   CU(cudaMemcpy(out64, c->d_prof.p, sizeof(long long) * 64, cudaMemcpyDeviceToHost));
+  return MVICP_OK;
+}
+// development aid: the per-edge output of the last LM evaluation, E x 160 doubles (EOUT), as lm_edge_kernel /
+// lm_edge_general_kernel wrote it and gather_blocks / gather_gradient / edge_cost_sum read it.  Edge e's record:
+//   [0, 144)    the 12x12 pair matrix Hp, row-major; rows and columns 0-5 are the src frame's tangent, 6-11 the dst frame's
+//               (lm_step's sub-blocks ss | sk over ks | kk)
+//   [144, 156)  the pair gradient: 6 src entries, then 6 dst entries
+//   156         the edge's cost, 1/2 sum rho(|r|^2) (1/2 sum |r|^2 without the loss);  157-159 zero
+// Each 6-vector is in the parameterisation's own tangent order: angle-axis (dw, dt), quaternion (dq, dt), SE3 (upsilon,
+// omega).  An edge whose src frame is fixed contributes nothing and reads as zeros: lm_edge_kernel writes zeros for it in a
+// joint solve, but in a component solve the edges of a component without a free frame belong to no problem and are never
+// written, so the readout zeroes every such record itself.  The blocks are those of the LAST evaluation: after
+// mvicp_optimize with max_num_iterations = 0 the start point; after a rejected step the rejected candidate.  The evaluation
+// enqueued behind a finished solve is skipped by its DoneGate and leaves them alone.  In a component solve each edge holds its
+// own problem's last evaluation.  MVICP_ERR_STATE before any LM solve has evaluated since the graph was set, after a g2o
+// solve, after a solve that failed, and in a sharded context.  Launches nothing and changes no state.
+int mvicp_debug_edge_blocks(mvicp_ctx* c, double* out, int64_t capacity, int32_t* n_edges) {
+  if (!c || !n_edges) return fail(MVICP_ERR_INVALID, "mvicp_debug_edge_blocks: bad arguments");
+  if (c->world > 1) return fail(MVICP_ERR_STATE, "mvicp_debug_edge_blocks: the context is sharded");
+  if (!c->lm_blocks_E || c->lm_blocks_E != c->E) return fail(MVICP_ERR_STATE, "mvicp_debug_edge_blocks: no completed LM solve since the graph was set");
+  *n_edges = c->E;
+  if (!out) return MVICP_OK;
+  if (capacity < (int64_t)EOUT * c->E) return fail(MVICP_ERR_INVALID, "mvicp_debug_edge_blocks: capacity %lld < %lld", (long long)capacity, (long long)EOUT * c->E);
+  CU(cudaSetDevice(c->device));
+  CU(cudaStreamSynchronize(c->stream));
+  CU(cudaMemcpy(out, c->d_eout.p, sizeof(double) * EOUT * c->E, cudaMemcpyDeviceToHost));
+  for (int e = 0; e < c->E; ++e)
+    if (c->lm_blocks_fixed[c->h_edges[e].src]) std::memset(out + (size_t)EOUT * e, 0, sizeof(double) * EOUT);
   return MVICP_OK;
 }
 int mvicp_get_stream(mvicp_ctx* c, void** stream) { if (!c || !stream) return fail(MVICP_ERR_INVALID, "bad arguments"); *stream = (void*)c->stream; return MVICP_OK; }
