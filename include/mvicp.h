@@ -230,8 +230,25 @@ int mvicp_optimize_g2o(mvicp_ctx* ctx, int32_t cost, const mvicp_g2o_options* op
 int mvicp_pairwise_g2o(const mvicp_config* cfg, int32_t cost, const double* src_xyz, const double* dst_xyz, const double* nor_xyz,
                        int64_t n, const mvicp_g2o_options* opt, double* pose16_out, mvicp_g2o_summary* summary);
 /* The trial trace of the last mvicp_optimize_g2o: 5 doubles per trial (lambda, chi, tchi, rho, accepted), in order.  Copies
- * min(capacity, recorded) rows; *n_trials = trials run (the first 65536 are recorded). */
+ * min(capacity, recorded) rows; *n_trials = trials run (the first 65536 are recorded).  After mvicp_optimize_g2o_components:
+ * MVICP_ERR_STATE (use mvicp_g2o_trace_component). */
 int mvicp_g2o_trace(mvicp_ctx* ctx, double* out5, int64_t capacity, int64_t* n_trials);
+/* One independent g2o solve per connected component (mvicp_get_components numbering), all in one pipelined loop: a batch of
+ * unrelated registrations in one context.  The lowest frame of every component is fixed (as frame 0 is by mvicp_optimize_g2o,
+ * icp-g2o.cpp:182-186); user-set flags are kept.  Each component is solved exactly as mvicp_optimize_g2o solves it in a fresh
+ * context holding only that component (frames ascending, edges in graph order, same fixed flags, correspondences and options):
+ * its own lambda, trials, calls, noImpr counter, ended / last_call_end and chi2; on a connected graph the result equals
+ * mvicp_optimize_g2o's bit for bit.  Shared by the batch: the streaming tile length (from all active correspondence slots) and
+ * the storage mode.  Argument checks are mvicp_optimize_g2o's, made before any state changes.  summaries (nullable):
+ * n_components entries; a component without a vertex gets mvicp_optimize_g2o's MVICP_G2O_END_NO_VERTICES summary and keeps its
+ * poses bit for bit.  chi2_per_call (nullable): n_components rows of (max_calls + 1) doubles, row k as mvicp_optimize_g2o fills
+ * it for component k (entries past calls + 1 unspecified).  Each problem of a batch of P records the first
+ * max(1024, 65536 / P) trials of its trace.  Sharded context: MVICP_ERR_STATE. */
+int mvicp_optimize_g2o_components(mvicp_ctx* ctx, int32_t cost, const mvicp_g2o_options* opt, mvicp_g2o_summary* summaries,
+                                  double* chi2_per_call);
+/* The trial trace of component k of the last g2o solve, as mvicp_g2o_trace returns a trace (k = 0 after mvicp_optimize_g2o,
+ * where it equals mvicp_g2o_trace).  k outside the last solve's components: MVICP_ERR_INVALID. */
+int mvicp_g2o_trace_component(mvicp_ctx* ctx, int32_t component, double* out5, int64_t capacity, int64_t* n_trials);
 
 /* One pass of the loop body main_multiview.cpp:150-169 (correspond + optimize). */
 int mvicp_icp_round(mvicp_ctx* ctx, float thresh, int32_t param, int32_t cost, int32_t robust,

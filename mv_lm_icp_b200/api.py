@@ -340,13 +340,37 @@ class Engine:
         d = s.asdict()
         return d, chi[:d["calls"] + 1].copy()
 
-    def g2o_trace(self):
-        """The last g2o solve's trials, one row each: lambda, chi, tchi, rho, accepted (mvicp_g2o_trace)."""
+    def optimize_g2o_components(self, cost=COST_P2PLANE, options=None):
+        """One independent g2o solve per connected component, all in one batched loop (mvicp_optimize_g2o_components): each
+        component ends exactly as optimize_g2o() would in an engine holding only that component.  Fixes the lowest frame of
+        every component.  Returns one (summary dict, chi2 before the first call and after every call) per component, in
+        component order."""
+        o = options if options is not None else default_g2o_options()
+        n = C.c_int32(0)
+        check(self._l.mvicp_get_components(self._ctx, C.byref(n), None))
+        K = n.value
+        s = (G2oSummary * max(1, K))(); chi = np.zeros((max(1, K), o.max_calls + 1))
+        check(self._l.mvicp_optimize_g2o_components(self._ctx, C.c_int32(cost), C.byref(o), s, _p(chi)))
+        out = []
+        for k in range(K):
+            d = s[k].asdict()
+            out.append((d, chi[k, :d["calls"] + 1].copy()))
+        return out
+
+    def g2o_trace(self, component=None):
+        """The last g2o solve's trials, one row each: lambda, chi, tchi, rho, accepted (mvicp_g2o_trace); with `component`,
+        that component's trials of the last solve (mvicp_g2o_trace_component).  One row per trial run; rows past the recorded
+        ones are zero."""
         n = C.c_int64(0)
-        check(self._l.mvicp_g2o_trace(self._ctx, None, C.c_int64(0), C.byref(n)))
+
+        def fetch(out, cap):
+            if component is None:
+                return self._l.mvicp_g2o_trace(self._ctx, out, C.c_int64(cap), C.byref(n))
+            return self._l.mvicp_g2o_trace_component(self._ctx, C.c_int32(component), out, C.c_int64(cap), C.byref(n))
+        check(fetch(None, 0))
         out = np.zeros((n.value, 5))
         if n.value:
-            check(self._l.mvicp_g2o_trace(self._ctx, _p(out), C.c_int64(n.value), C.byref(n)))
+            check(fetch(_p(out), n.value))
         return out
 
     def recompute_normals(self, k=10, fetch=True):

@@ -1,8 +1,10 @@
-"""Rate of the per-component LM solve (mvicp_optimize_components): ICP rounds of correspond + optimize_components on a batch of
-independent registrations, against one context per component run one after another, and against the joint optimize over
-their union (a different problem: one trust region for all; shown for time only).
+"""Rate of the per-component solves (mvicp_optimize_components, mvicp_optimize_g2o_components): ICP rounds of correspond +
+optimize_components (--solver lm) or correspond + optimize_g2o_components (--solver g2o) on a batch of independent
+registrations, against one context per component run one after another, and against the joint optimize / optimize_g2o over
+their union (a different problem: one trust region / one lambda for all; shown for time only).
 
-  python tools/bench_components.py [--workload pairs|real|3|all] [--rounds K] [--warmup W] [--reps R] [--pairs B] [--points N]
+  python tools/bench_components.py [--solver lm|g2o] [--workload pairs|real|3|all] [--rounds K] [--warmup W] [--reps R]
+                                   [--pairs B] [--points N]
 
 Workloads: `pairs` = B synthetic two-view problems of N points (8 distinct scenes, each pair from its own perturbed start);
 `real` = the 18 Bunny_RealData frames of tests/golden/bunny18.npz (recomputed normals) cut into 9 pairs (2i, 2i + 1);
@@ -10,8 +12,10 @@ Workloads: `pairs` = B synthetic two-view problems of N points (8 distinct scene
 three arms alternate R times in one process; each run resets the poses, runs W rounds untimed and then K timed rounds (wall
 clock between stream synchronisations).  The batched and the sequential arm must give the same poses per component: bit for bit
 when the component's own context picks the batch's streaming tile length (the batch picks it from all components'
-correspondence slots), else within 1e-12 relative; otherwise the tool exits with an error after its JSON line.  Prints one JSON
-line with the card and its power limit."""
+correspondence slots), else (LM) within 1e-12 relative; otherwise the tool exits with an error after its JSON line.  g2o's
+rho > 0 and impr > 0 decisions are taken at rounding level near convergence (DESIGN section 2), so where the tile lengths differ
+the g2o arms are only reported (largest relative pose and final chi2 difference), never failed.  g2o: the solver's defaults
+(optimize(100) calls until noImpr passes 5).  Prints one JSON line with the card and its power limit."""
 import argparse
 import json
 import os
@@ -89,21 +93,27 @@ def engine(mv, c, recompute):
     return eng
 
 
-def run(engs, comps_of_eng, arm, rounds, warmup, mv, cutoff):
-    """One run of an arm: reset poses, warm up, time `rounds` rounds; returns (seconds, final poses per engine)."""
+def run(engs, comps_of_eng, arm, rounds, warmup, mv, cutoff, solver="lm"):
+    """One run of an arm: reset poses, warm up, time `rounds` rounds; returns (seconds, final poses per engine, g2o: the last
+    round's final chi2 per component of every engine)."""
     for eng, c in zip(engs, comps_of_eng):
         fx = [0] * len(c["pts"])
         for f in c.get("lowest", [0]):
             fx[f] = 1
         eng.set_poses(c["poses"], fx)
     total = 0.0
+    chi = [[] for _ in engs]
     for r in range(warmup + rounds):
         for eng in engs:
             eng.sync()
         t0 = time.perf_counter()
-        for eng in engs:
+        for i, eng in enumerate(engs):
             eng.correspond(cutoff)
-            if arm == "batched":
+            if solver == "g2o" and arm == "batched":
+                chi[i] = [s["chi2_final"] for s, _ in eng.optimize_g2o_components(mv.COST_P2PLANE)]
+            elif solver == "g2o":
+                chi[i] = [eng.optimize_g2o(mv.COST_P2PLANE)[0]["chi2_final"]]
+            elif arm == "batched":
                 eng.optimize_components(mv.PARAM_SE3, mv.COST_P2PLANE, True)
             else:
                 eng.optimize(mv.PARAM_SE3, mv.COST_P2PLANE, True)
@@ -111,7 +121,7 @@ def run(engs, comps_of_eng, arm, rounds, warmup, mv, cutoff):
             eng.sync()
         if r >= warmup:
             total += time.perf_counter() - t0
-    return total, [eng.get_poses() for eng in engs]
+    return total, [eng.get_poses() for eng in engs], chi
 
 
 def card():
@@ -135,37 +145,46 @@ def bench_workload(name, args):
             "joint": [engine(mv, u, recompute)]}
     ctx = {"batched": [u_batched], "sequential": comps, "joint": [dict(u, lowest=first)]}
     times = {a: [] for a in engs}
-    poses = {}
+    poses, chis = {}, {}
     for _ in range(args.reps):
         for arm in ("batched", "sequential", "joint"):
-            t, P = run(engs[arm], ctx[arm], arm, args.rounds, args.warmup, mv, bench.CUTOFF)
-            times[arm].append(t); poses[arm] = P
+            t, P, chi = run(engs[arm], ctx[arm], arm, args.rounds, args.warmup, mv, bench.CUTOFF, args.solver)
+            times[arm].append(t); poses[arm] = P; chis[arm] = chi
     # per component: bit for bit when its own context picks the batch's streaming tile, else within POSE_TOL (the tile fixes
     # how the edge sums are associated)
     Pb = poses["batched"][0]
     tl_batch = tile_len(sum(active_slots(c) for c in comps))
-    diff, bitwise, ok, tiles = 0.0, True, True, set()
-    for c, f0, Ps in zip(comps, first, poses["sequential"]):
+    diff, chi_diff, bitwise, ok, tiles = 0.0, 0.0, True, True, set()
+    for k, (c, f0, Ps) in enumerate(zip(comps, first, poses["sequential"])):
         a, b = Pb[f0:f0 + len(c["pts"])], Ps
         same = np.array_equal(a.view(np.uint64), b.view(np.uint64))
         rel = float(np.max(np.abs(a - b)) / max(1.0, np.max(np.abs(b))))
         tl = tile_len(active_slots(c)); tiles.add(tl)
-        ok = ok and (same if tl == tl_batch else rel <= POSE_TOL)
+        if args.solver == "g2o":
+            cb, cs = chis["batched"][0][k], chis["sequential"][k][0]
+            same = same and np.float64(cb).view(np.uint64) == np.float64(cs).view(np.uint64)
+            chi_diff = max(chi_diff, abs(cb - cs) / max(abs(cs), 1e-300))
+            ok = ok and (same or tl != tl_batch)
+        else:
+            ok = ok and (same if tl == tl_batch else rel <= POSE_TOL)
         bitwise = bitwise and same
         diff = max(diff, rel)
     rate = {a: [round(args.rounds / t, 3) for t in ts] for a, ts in times.items()}
     for es in engs.values():
         for e in es:
             e.close()
-    return {"workload": name, "components": len(comps), "frames": len(u["pts"]),
+    agree = {"ok": bool(ok), "bitwise": bool(bitwise), "max_rel_diff": diff, "tile_batched": tl_batch, "tile_sequential": sorted(tiles)}
+    if args.solver == "g2o":
+        agree["max_rel_chi2_diff"] = chi_diff
+    return {"workload": name, "solver": args.solver, "components": len(comps), "frames": len(u["pts"]),
             "rounds_per_s": rate, "median_rounds_per_s": {a: float(np.median(v)) for a, v in rate.items()},
             "speedup_vs_sequential": float(np.median(rate["batched"]) / np.median(rate["sequential"])),
-            "poses_batched_vs_sequential": {"ok": bool(ok), "bitwise": bool(bitwise), "max_rel_diff": diff, "tile_batched": tl_batch,
-                                            "tile_sequential": sorted(tiles)}}
+            "poses_batched_vs_sequential": agree}
 
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--solver", default="lm", choices=["lm", "g2o"])
     ap.add_argument("--workload", default="all", choices=["pairs", "real", "3", "all"])
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=1)
@@ -175,7 +194,9 @@ def main():
     args = ap.parse_args()
     names = ["pairs", "real", "3"] if args.workload == "all" else [args.workload]
     gpu, power_limit = card()
-    out = {"metric": "ICP rounds per second, correspond + optimize_components vs one context per component vs joint optimize",
+    metric = {"lm": "correspond + optimize_components vs one context per component vs joint optimize",
+              "g2o": "correspond + optimize_g2o_components vs one context per component vs joint optimize_g2o"}[args.solver]
+    out = {"metric": "ICP rounds per second, " + metric,
            "gpu": gpu, "power_limit": power_limit, "rounds": args.rounds, "warmup": args.warmup, "reps": args.reps,
            "results": [bench_workload(n, args) for n in names]}
     print(json.dumps(out))
