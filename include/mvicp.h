@@ -184,6 +184,35 @@ int mvicp_get_components(mvicp_ctx* ctx, int32_t* n_components, int32_t* compone
 int mvicp_optimize_components(mvicp_ctx* ctx, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt,
                               mvicp_lm_summary* summaries);
 
+/* Pose covariances of the LM problem (ceres::Covariance, DESIGN.md section 6j): C = (J^T J)^-1 at the CURRENT poses, for the
+ * problem mvicp_optimize(param, cost, robust) would solve now -- the current correspondences and edge weights, frame 0 and every
+ * flagged frame fixed, the edges of fixed src frames inactive, the unit or general eval path chosen as the solve chooses it.
+ * J^T J is the matrix of the solve's first evaluation, with the loss applied as Ceres applies it (apply_loss_function = true;
+ * SoftL1: rows scaled by sqrt(rho')).  After mvicp_optimize_components the lowest frame of every component is flagged, so the
+ * call covers such a batch as it stands.
+ *   cov36[36 k .. 36 k + 36): Cov(x_a, x_b), a = frame_a[k], b = frame_b[k], 6x6 row-major, in the local tangent of the solve
+ * (and of mvicp_debug_edge_blocks), what Ceres >= 1.14's GetCovarianceBlockInTangentSpace returns for the reference's blocks:
+ *   MVICP_PARAM_SE3   (upsilon, omega) of x exp(delta), Sophus order;
+ *   MVICP_PARAM_QUAT  (dq, dt): EigenQuaternionParameterization's dq (x, y, z), then the translation;
+ *   MVICP_PARAM_AA    (dw, dt): angle-axis, then the translation.
+ *   status[k] (nullable), in this order of precedence:
+ *     MVICP_COV_FIXED        a or b is fixed: zeros (Ceres gives constant blocks zero covariance);
+ *     MVICP_COV_INDEPENDENT  a and b lie in different connected components (mvicp_get_components): zeros, since J^T J is
+ *                            block-diagonal over the components;
+ *     MVICP_COV_SINGULAR     their component is rank-deficient: NaN.  A component without a fixed frame always is (its gauge
+ *                            is free); otherwise the rank rule [ext, not Ceres' QR rule]: with S = diag(1 / sqrt(H_jj)) and the
+ *                            Cholesky factor L~ of S H S, singular if some H_jj is zero or not finite, a pivot is not positive
+ *                            or not finite, or L~_jj^2 <= 64 n 2^-53 (n unknowns of the component);
+ *     MVICP_COV_OK           the block of C = S (S H S)^-1 S, each component factored as a problem of its own.
+ * A block's bits depend only on the problem: not on which other pairs are requested, their order or duplicates; (b, a) is
+ * the exact transpose of (a, b), so a diagonal block is exactly symmetric; two calls give the same bytes.  The call changes no
+ * pose, fixed flag, correspondence, certificate, cached LM / g2o layout or statistic other than kernel_launches.
+ * MVICP_ERR_INVALID before any work: bad param / cost, n_pairs < 0, a null array with n_pairs > 0, a frame outside [0, M),
+ * point-to-plane without normals.  MVICP_ERR_STATE: no frames or graph, or a sharded context (the call runs on one GPU). */
+enum { MVICP_COV_OK = 0, MVICP_COV_FIXED = 1, MVICP_COV_INDEPENDENT = 2, MVICP_COV_SINGULAR = 3 };
+int mvicp_covariance(mvicp_ctx* ctx, int32_t param, int32_t cost, int32_t robust, int32_t n_pairs, const int32_t* frame_a,
+                     const int32_t* frame_b, double* cov36, int32_t* status);
+
 /* ICP_G2O::g2oOptimizer (include/icp-g2o.h:14, icp-g2o.cpp:149-303), the --g2o path of main_multiview.cpp:158-164: one g2o
  * Edge_V_V_GICP per stored correspondence of every edge with a free end (vertex 0 = dst, vertex 1 = src), VertexSE3 poses,
  * Levenberg-Marquardt over H + lambda I (no Jacobi scaling), and the reference's outer loop of optimize(iterations_per_call)

@@ -66,7 +66,10 @@ EXPORTS = ["mvicp_default_lm_options", "mvicp_last_error", "mvicp_create", "mvic
            "mvicp_default_g2o_options", "mvicp_optimize_g2o", "mvicp_pairwise_g2o", "mvicp_g2o_trace",
            "mvicp_closest_points", "mvicp_set_frames_device", "mvicp_set_edge_device", "mvicp_get_all_edges_device",
            "mvicp_closest_points_device", "mvicp_get_normals_device", "mvicp_knn_self_device",
-           "mvicp_get_components", "mvicp_optimize_components", "mvicp_optimize_g2o_components", "mvicp_g2o_trace_component"]
+           "mvicp_get_components", "mvicp_optimize_components", "mvicp_optimize_g2o_components", "mvicp_g2o_trace_component",
+           "mvicp_covariance"]
+
+COV_OK, COV_FIXED, COV_INDEPENDENT, COV_SINGULAR = 0, 1, 2, 3   # mvicp_covariance's per-pair status (MVICP_COV_*)
 
 
 def build(force=False):

@@ -15,7 +15,7 @@ import sys
 import numpy as np
 
 from . import _lib
-from ._lib import Config, G2oOptions, G2oSummary, LmOptions, LmSummary, Stats, check
+from ._lib import COV_FIXED, COV_INDEPENDENT, COV_OK, COV_SINGULAR, Config, G2oOptions, G2oSummary, LmOptions, LmSummary, Stats, check  # noqa: F401
 
 PARAM_AA, PARAM_QUAT, PARAM_SE3 = 0, 1, 2
 COST_P2P, COST_P2PLANE, COST_MIXED = 0, 1, 2
@@ -324,6 +324,23 @@ class Engine:
         check(self._l.mvicp_optimize_components(self._ctx, C.c_int32(param), C.c_int32(cost), C.c_int32(int(robust)),
                                                 C.byref(options) if options is not None else None, s))
         return [s[k].asdict() for k in range(n.value)]
+
+    def covariance(self, pairs=None, param=PARAM_SE3, cost=COST_P2PLANE, robust=True):
+        """Covariance blocks of the problem optimize(param, cost, robust) would solve now, at the current poses
+        (mvicp_covariance, ceres::Covariance in the parameterisation's tangent space): `pairs` is a list of (a, b) frame pairs,
+        None for the diagonal block of every frame.  Returns (cov float64 [n, 6, 6], status int32 [n]) with cov[k] = Cov(x_a,
+        x_b); status COV_OK, COV_FIXED (zeros), COV_INDEPENDENT (different components: zeros) or COV_SINGULAR (NaN)."""
+        if pairs is None:
+            pairs = [(f, f) for f in range(self.M)]
+        p = np.asarray(pairs, np.int64).reshape(-1, 2)
+        if p.size and (p.min() < -2**31 or p.max() >= 2**31):
+            raise _lib.MvicpError(1, "covariance: frame index out of range")
+        a = np.ascontiguousarray(p[:, 0], np.int32); b = np.ascontiguousarray(p[:, 1], np.int32)
+        n = len(a)
+        cov = np.zeros((n, 6, 6)); st = np.zeros(n, np.int32)
+        check(self._l.mvicp_covariance(self._ctx, C.c_int32(param), C.c_int32(cost), C.c_int32(int(robust)), C.c_int32(n),
+                                       _p(a, C.c_int32), _p(b, C.c_int32), _p(cov), _p(st, C.c_int32)))
+        return cov, st
 
     def icp_round(self, thresh=0.05, param=PARAM_SE3, cost=COST_P2PLANE, robust=True, options=None):
         s = LmSummary()

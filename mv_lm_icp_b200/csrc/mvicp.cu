@@ -24,6 +24,7 @@
 #include "../../include/mvicp.h"
 #include "closed.cuh"
 #include "compact.cuh"
+#include "covariance.cuh"
 #include "device_io.cuh"
 #include "far.cuh"
 #include "g2o.cuh"
@@ -73,6 +74,16 @@ struct DevBuf {
   }
   void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
   template <typename T> T* as() const { return reinterpret_cast<T*>(p); }
+};
+
+// LM problems as upload_problems lays them out: one int32 buffer (frame and edge lists, gather lists, envelopes, skylines, the
+// edge -> problem map), one fp64 buffer, the LmProblem views (device, and a host copy), room for P + 1 states
+struct ProblemBufs {
+  DevBuf i32, f64, prob, state;
+  std::vector<LmProblem> h_prob;           // host copy of the views
+  const int32_t* edge_prob = nullptr;      // [E] edge -> problem, or -1 (in i32)
+  size_t dyn = 0;                          // dynamic shared memory of the step kernels: the maximum over the problems
+  std::vector<uint8_t> key;                // kind of solve, fixed flags and graph generation the problems were uploaded for
 };
 
 struct mvicp_ctx {
@@ -125,12 +136,14 @@ struct mvicp_ctx {
   std::vector<int32_t> h_col;
   volatile int32_t* h_flag = nullptr; volatile int32_t* d_flag = nullptr;   // mapped pinned ring written by the step kernels
   uint32_t graph_gen = 0;
-  // the LM problems last uploaded (upload_problems): int32 lists, fp64 arrays, LmProblem views, states, the step kernel's ticket
-  DevBuf d_lm_i32, d_lm_f64, d_lm_prob, d_lm_state, d_lm_ticket;
-  std::vector<LmProblem> h_prob;           // host copy of the views
-  const int32_t* lm_edge_prob = nullptr;   // [E] edge -> problem, or -1 (in d_lm_i32)
-  size_t lm_dyn = 0;                       // dynamic shared memory of the step kernels: the maximum over the problems
-  std::vector<uint8_t> layout_key;         // kind of solve, fixed flags and graph generation the problems were uploaded for
+  // the LM problems last uploaded for a solve (upload_problems), and the step kernel's ticket
+  ProblemBufs lm;
+  DevBuf d_lm_ticket;
+  // mvicp_covariance: its own problems (cached like lm), evaluation point, tiles, pair matrices and outputs, so that nothing a
+  // solve or mvicp_debug_edge_blocks reads is touched
+  ProblemBufs cov;
+  DevBuf d_cov_x, d_cov_cand, d_cov_Rt, d_cov_K, d_cov_gen, d_cov_partial, d_cov_eout, d_cov_tiles, d_cov_etb, d_cov_status,
+         d_cov_jobs, d_cov_out;
   void* h_state = nullptr; size_t h_state_cap = 0;   // pinned staging of the P + 1 LmStates
   // g2o solve (g2o.cuh); the normal equations of its problems are uploaded LM problems
   DevBuf d_g2o_state, d_g2o_prob, d_g2o_x, d_g2o_ev, d_g2o_nop, d_g2o_chi, d_g2o_trace, d_g2o_tiles, d_g2o_tile_begin, d_g2o_cnt;
@@ -607,6 +620,13 @@ int mvicp_get_poses(mvicp_ctx* c, double* poses16) {
   return MVICP_OK;
 }
 
+// LM streaming tile length for this many active correspondence slots (edges of free src frames, over all ranks)
+static int eval_tile_len_of(int64_t active_slots) {
+  int tl = 8192;
+  while (tl > 1024 && active_slots / tl < 8 * NUM_SMS) tl >>= 1;
+  return tl;
+}
+
 // edge ownership, slot offsets and the tile lists of the NN / LM streaming kernels: depends on the graph, the cloud sizes, the
 // fixed flags and the rank layout -- not on the correspondences, which keep their slots
 static int layout_work(mvicp_ctx* c) {
@@ -628,8 +648,7 @@ static int layout_work(mvicp_ctx* c) {
   // (bench.py checks that in every multi-GPU run; round 1 chose it from the rank's own share and was not).
   int64_t active_slots = 0;
   for (int e = 0; e < E; ++e) if (c->edge_owner[e] >= 0) active_slots += c->h_edges[e].n_src;
-  int tl = 8192;
-  while (tl > 1024 && active_slots / tl < 8 * NUM_SMS) tl >>= 1;
+  const int tl = eval_tile_len_of(active_slots);
   c->eval_tile_len = tl;
   (void)owned_slots;
   std::vector<Tile> kt, et; std::vector<int32_t> etb(E + 1, 0);
@@ -1093,13 +1112,13 @@ int mvicp_closest_points_device(mvicp_ctx* c, int32_t frame, const double* q, in
 // factor, and zeroes the dense normal matrix.
 //
 // plan_normal_layout is the host half for one problem: `frames` (ascending) are its frames, local frame i being frames[i], and
-// `edges` its edges in graph order; c->h_col holds the local columns (n of them).  The gather lists name graph edges.
+// `edges` its edges in graph order; hcol holds the local columns (n of them).  The gather lists name graph edges.
 struct LayoutPlan {
   std::vector<int32_t> col, hb_ptr{0}, hb_row, hb_col, hc_edge, hc_sub, gb_ptr{0}, gc_edge, gc_side, rlast, rfirst, rowbase;
   int64_t l_size = 0;        // doubles of the factor's skyline storage (row profiles + rhs row)
 };
-static int plan_normal_layout(const mvicp_ctx* c, const std::vector<int32_t>& frames, const std::vector<int32_t>& edges, int n,
-                              const std::vector<uint8_t>& active, LayoutPlan& p) {
+static int plan_normal_layout(const mvicp_ctx* c, const std::vector<int32_t>& hcol, const std::vector<int32_t>& frames,
+                              const std::vector<int32_t>& edges, int n, const std::vector<uint8_t>& active, LayoutPlan& p) {
   const int M = (int)frames.size();
   std::vector<int32_t> loc(c->M, -1);
   for (int i = 0; i < M; ++i) loc[frames[i]] = i;
@@ -1107,13 +1126,13 @@ static int plan_normal_layout(const mvicp_ctx* c, const std::vector<int32_t>& fr
   for (const int e : edges) {
     if (!active[e]) continue;
     const int s = loc[c->h_edges[e].src], k = loc[c->h_edges[e].dst];
-    const bool fs = c->h_col[frames[s]] >= 0, fk = c->h_col[frames[k]] >= 0;
+    const bool fs = hcol[frames[s]] >= 0, fk = hcol[frames[k]] >= 0;
     if (fs) { blk[(size_t)s * M + s].push_back({e, 0}); gl[s].push_back({e, 0}); }
     if (fs && fk) { blk[(size_t)s * M + k].push_back({e, 1}); blk[(size_t)k * M + s].push_back({e, 2}); }
     if (fk) { blk[(size_t)k * M + k].push_back({e, 3}); gl[k].push_back({e, 1}); }
   }
   p.col.resize(M);
-  for (int i = 0; i < M; ++i) p.col[i] = c->h_col[frames[i]];
+  for (int i = 0; i < M; ++i) p.col[i] = hcol[frames[i]];
   for (int r = 0; r < M; ++r)
     for (int q = 0; q < M; ++q) {
       const auto& l = blk[(size_t)r * M + q];
@@ -1142,18 +1161,19 @@ static int plan_normal_layout(const mvicp_ctx* c, const std::vector<int32_t>& fr
   return MVICP_OK;
 }
 
-// The LM problems, problem q over frames[q] and edges[q] with the local columns in c->h_col, laid out by plan_normal_layout and
-// uploaded end to end: one int32 buffer (frame and edge lists, gather lists, envelopes, skylines, then the edge -> problem map),
-// one fp64 buffer (per problem H, Hc | g, gc, scale, diag, step, rhs | factor; Sigma n^2, not (Sigma n)^2), the LmProblem views,
-// room for P + 1 states ([P]: the whole graph, for lm_init_kernel) and the step kernel's ticket.  `key` names what was uploaded.
-static int upload_problems(mvicp_ctx* c, const std::vector<std::vector<int32_t>>& frames, const std::vector<std::vector<int32_t>>& edges,
-                           const std::vector<uint8_t>& active, const std::vector<uint8_t>& key) {
+// The LM problems, problem q over frames[q] and edges[q] with the local columns in hcol, laid out by plan_normal_layout and
+// uploaded end to end into pb: one int32 buffer (frame and edge lists, gather lists, envelopes, skylines, then the edge -> problem
+// map), one fp64 buffer (per problem H, Hc | g, gc, scale, diag, step, rhs | factor; Sigma n^2, not (Sigma n)^2), the LmProblem
+// views, room for P + 1 states ([P]: the whole graph, for lm_init_kernel), the step kernel's ticket and the pair matrices' buffer
+// d_eout.  `key` names what was uploaded.
+static int upload_problems(mvicp_ctx* c, ProblemBufs& pb, const std::vector<int32_t>& hcol, const std::vector<std::vector<int32_t>>& frames,
+                           const std::vector<std::vector<int32_t>>& edges, const std::vector<uint8_t>& active, const std::vector<uint8_t>& key) {
   const int P = (int)frames.size(), E = c->E;
-  c->layout_key.clear();   // the buffers below change before the new views are complete
+  pb.key.clear();   // the buffers below change before the new views are complete
   std::vector<LayoutPlan> plans(P); std::vector<int> ns(P, 0);
   for (int q = 0; q < P; ++q) {
-    for (int f : frames[q]) if (c->h_col[f] >= 0) ns[q] += 6;
-    RET(plan_normal_layout(c, frames[q], edges[q], ns[q], active, plans[q]));
+    for (int f : frames[q]) if (hcol[f] >= 0) ns[q] += 6;
+    RET(plan_normal_layout(c, hcol, frames[q], edges[q], ns[q], active, plans[q]));
   }
   std::vector<int32_t> blob;
   auto put = [&](const std::vector<int32_t>& v) { const size_t o = blob.size(); blob.insert(blob.end(), v.begin(), v.end()); return o; };
@@ -1169,10 +1189,10 @@ static int upload_problems(mvicp_ctx* c, const std::vector<std::vector<int32_t>>
   const size_t edge_map = put(prob_of_edge);
   std::vector<size_t> fo(P + 1, 0);
   for (int q = 0; q < P; ++q) { const size_t n = ns[q]; fo[q + 1] = fo[q] + 2 * n * n + 6 * n + (size_t)plans[q].l_size; }
-  RET(c->d_lm_i32.reserve(sizeof(int32_t) * blob.size()));
-  RET(c->d_lm_f64.reserve(sizeof(double) * fo[P]));
-  RET(c->d_lm_prob.reserve(sizeof(LmProblem) * P));
-  RET(c->d_lm_state.reserve(sizeof(LmState) * (P + 1)));
+  RET(pb.i32.reserve(sizeof(int32_t) * blob.size()));
+  RET(pb.f64.reserve(sizeof(double) * fo[P]));
+  RET(pb.prob.reserve(sizeof(LmProblem) * P));
+  RET(pb.state.reserve(sizeof(LmState) * (P + 1)));
   RET(c->d_lm_ticket.reserve(sizeof(unsigned int)));
   RET(c->d_eout.reserve(sizeof(double) * EOUT * E));
   if (c->h_state_cap < (size_t)P + 1) {
@@ -1181,14 +1201,14 @@ static int upload_problems(mvicp_ctx* c, const std::vector<std::vector<int32_t>>
     CU(cudaMallocHost(&c->h_state, sizeof(LmState) * (P + 1)));
     c->h_state_cap = P + 1;
   }
-  const int32_t* ib = c->d_lm_i32.as<int32_t>();
+  const int32_t* ib = pb.i32.as<int32_t>();
   std::vector<LmProblem> probs(P);
   size_t dyn = 0;
   for (int q = 0; q < P; ++q) {
     const int n = ns[q]; const Off& o = io[q];
     LmProblem& p = probs[q];
     std::memset(&p, 0, sizeof p);
-    p.S = c->d_lm_state.as<LmState>() + q;
+    p.S = pb.state.as<LmState>() + q;
     p.frame = ib + o.frame; p.edge = ib + o.edge;
     NormalLayout& l = p.lay;
     l.col = ib + o.col;
@@ -1196,7 +1216,7 @@ static int upload_problems(mvicp_ctx* c, const std::vector<std::vector<int32_t>>
     l.n_hblocks = (int32_t)plans[q].hb_row.size();
     l.gb_ptr = ib + o.gb_ptr; l.gc_edge = ib + o.gc_edge; l.gc_side = ib + o.gc_side;
     l.rlast = ib + o.rlast; l.rfirst = ib + o.rfirst; l.rowbase = ib + o.rowbase;
-    double* d = c->d_lm_f64.as<double>() + fo[q];
+    double* d = pb.f64.as<double>() + fo[q];
     p.H = d; d += (size_t)n * n; p.Hc = d; d += (size_t)n * n;
     p.g = d; d += n; p.gc = d; d += n; p.scale = d; d += n; p.diag = d; d += n; p.step = d; d += n; l.rhs = d; d += n;
     l.Lg = d;
@@ -1206,40 +1226,47 @@ static int upload_problems(mvicp_ctx* c, const std::vector<std::vector<int32_t>>
     l.l_in_smem = lb + vec <= 220 * 1024 ? 1 : 0;
     dyn = std::max(dyn, vec + (l.l_in_smem ? lb : 0));
   }
-  CU(cudaMemcpyAsync(c->d_lm_i32.p, blob.data(), sizeof(int32_t) * blob.size(), cudaMemcpyHostToDevice, c->stream));
-  CU(cudaMemcpyAsync(c->d_lm_prob.p, probs.data(), sizeof(LmProblem) * P, cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemcpyAsync(pb.i32.p, blob.data(), sizeof(int32_t) * blob.size(), cudaMemcpyHostToDevice, c->stream));
+  CU(cudaMemcpyAsync(pb.prob.p, probs.data(), sizeof(LmProblem) * P, cudaMemcpyHostToDevice, c->stream));
   // the step kernels write only the listed blocks of H and Hc; everything else stays zero from here
-  CU(cudaMemsetAsync(c->d_lm_f64.p, 0, sizeof(double) * fo[P], c->stream));
+  CU(cudaMemsetAsync(pb.f64.p, 0, sizeof(double) * fo[P], c->stream));
   CU(cudaMemsetAsync(c->d_lm_ticket.p, 0, sizeof(unsigned int), c->stream));
   CU(cudaStreamSynchronize(c->stream));   // the host vectors above must outlive their copies
-  c->h_prob = std::move(probs); c->lm_edge_prob = ib + edge_map; c->lm_dyn = dyn; c->layout_key = key;
+  pb.h_prob = std::move(probs); pb.edge_prob = ib + edge_map; pb.dyn = dyn; pb.key = key;
   return MVICP_OK;
 }
 }  // extern "C"
-template <bool F32> static void launch_eval(mvicp_ctx* c, int cost, int robust, DoneGate gate) {
-  const int nt = c->n_eval_tiles;
+// What one streaming evaluation reads and writes besides the frames, edges and correspondences: the tiles, the evaluation point
+// (per-frame Rt for the unit path, FrameGen for the general one) and the per-tile partials.  The solves use the context's own
+// (lm_eval_args); mvicp_covariance brings its own.
+struct EvalArgs { const Tile* tiles; int nt, tile_len; const Rt* Rt_; const FrameGen* gen; double* partial; };
+static EvalArgs lm_eval_args(mvicp_ctx* c) {
+  return EvalArgs{c->d_eval_tiles.as<Tile>(), c->n_eval_tiles, c->eval_tile_len, c->d_Rt.as<Rt>(), c->d_gen.as<FrameGen>(), c->d_partial.as<double>()};
+}
+template <bool F32> static void launch_eval(mvicp_ctx* c, const EvalArgs& a, int cost, int robust, DoneGate gate) {
+  const int nt = a.nt;
   if (!nt) return;
 #define MV_EVAL(NF, COSTK)                                                                                       \
   lm_eval_kernel<F32, NF, COSTK><<<nt, EVAL_THREADS, 0, c->stream>>>(                                            \
-      c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_eval_tiles.as<Tile>(), c->eval_tile_len,       \
-      c->d_corr.as<int32_t>(), c->d_Rt.as<Rt>(), c->d_weight.as<float>(), robust, c->d_partial.as<double>(), gate)
+      c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), a.tiles, a.tile_len,                                \
+      c->d_corr.as<int32_t>(), a.Rt_, c->d_weight.as<float>(), robust, a.partial, gate)
 #define MV_EVALC(NF) { if (cost == COST_P2P) MV_EVAL(NF, COST_P2P); else if (cost == COST_P2PLANE) MV_EVAL(NF, COST_P2PLANE); else MV_EVAL(NF, COST_MIXED); }
   if (F32 && c->nor_f32) MV_EVALC(F32) else MV_EVALC(false)
 #undef MV_EVALC
 #undef MV_EVAL
 }
 
-template <bool F32> static void launch_eval_general(mvicp_ctx* c, int param, int cost, int robust, DoneGate gate) {
+template <bool F32> static void launch_eval_general(mvicp_ctx* c, const EvalArgs& a, int param, int cost, int robust, DoneGate gate) {
   const int rot0 = param == PARAM_QUAT ? 0 : 3;   // tangent order: quaternion (rotation, translation), SE3 (translation, rotation)
-  const int nt = c->n_eval_tiles;
+  const int nt = a.nt;
   if (!nt) return;
 #define MV_EVALG(COSTK)                                                                                          \
   if (F32 && c->nor_f32) lm_eval_general_kernel<F32, F32, COSTK><<<nt, EVAL_THREADS, 0, c->stream>>>(        \
-      c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_eval_tiles.as<Tile>(), c->eval_tile_len,       \
-      c->d_corr.as<int32_t>(), c->d_gen.as<FrameGen>(), c->d_weight.as<float>(), robust, rot0, c->d_partial.as<double>(), gate); \
+      c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), a.tiles, a.tile_len,                                \
+      c->d_corr.as<int32_t>(), a.gen, c->d_weight.as<float>(), robust, rot0, a.partial, gate);                   \
   else lm_eval_general_kernel<F32, false, COSTK><<<nt, EVAL_THREADS, 0, c->stream>>>(                        \
-      c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), c->d_eval_tiles.as<Tile>(), c->eval_tile_len,       \
-      c->d_corr.as<int32_t>(), c->d_gen.as<FrameGen>(), c->d_weight.as<float>(), robust, rot0, c->d_partial.as<double>(), gate)
+      c->d_frames.as<FrameDev>(), c->d_edges.as<EdgeDev>(), a.tiles, a.tile_len,                                \
+      c->d_corr.as<int32_t>(), a.gen, c->d_weight.as<float>(), robust, rot0, a.partial, gate)
   if (cost == COST_P2P) { MV_EVALG(COST_P2P); } else if (cost == COST_P2PLANE) { MV_EVALG(COST_P2PLANE); } else { MV_EVALG(COST_MIXED); }
 #undef MV_EVALG
 }
@@ -1400,10 +1427,10 @@ static int solve_lm(mvicp_ctx* c, bool per_component, const char* fn, int32_t pa
   // the layout depends only on the kind of solve, the graph and the fixed flags: build and upload it when those change
   std::vector<uint8_t> key(c->fixed); key.push_back((uint8_t)(c->graph_gen & 0xff)); key.push_back((uint8_t)((c->graph_gen >> 8) & 0xff));
   key.push_back(per_component ? 1 : 0);
-  if (key != c->layout_key) {
+  if (key != c->lm.key) {
     std::vector<uint8_t> active(E);
     for (int e = 0; e < E; ++e) active[e] = !c->fixed[c->h_edges[e].src];
-    RET(upload_problems(c, pf, pe, active, key));
+    RET(upload_problems(c, c->lm, c->h_col, pf, pe, active, key));
   }
   LmState* st = static_cast<LmState*>(c->h_state);   // pinned staging: no synchronisation needed before the kernels
   std::memset(st, 0, sizeof(LmState) * (P + 1));
@@ -1414,7 +1441,7 @@ static int solve_lm(mvicp_ctx* c, bool per_component, const char* fn, int32_t pa
     s.M = (int32_t)pf[q].size(); s.E = (int32_t)pe[q].size(); s.n = ns[q]; s.F = s.n / 6;
     s.radius = opt.initial_trust_region_radius; s.decrease_factor = 2.0;
   }
-  LmState* dS = c->d_lm_state.as<LmState>();
+  LmState* dS = c->lm.state.as<LmState>();
   CU(cudaMemcpyAsync(dS, st, sizeof(LmState) * (P + 1), cudaMemcpyHostToDevice, c->stream));
   // the per-frame arrays of the evaluation point are shared by every problem (indexed by graph frame)
   RET(c->d_x.reserve(sizeof(double) * 7 * M)); RET(c->d_cand.reserve(sizeof(double) * 7 * M));
@@ -1430,7 +1457,7 @@ static int solve_lm(mvicp_ctx* c, bool per_component, const char* fn, int32_t pa
   w.G_eval = general ? c->d_gen.as<FrameGen>() : nullptr;
   w.x = c->d_x.as<double>(); w.cand = c->d_cand.as<double>(); w.Rt_eval = c->d_Rt.as<Rt>(); w.K_eval = c->d_K.as<double>();
   w.poses16 = c->d_poses.as<double>(); w.host_flag = c->d_flag;
-  const LmProblem* probs = c->d_lm_prob.as<LmProblem>();
+  const LmProblem* probs = c->lm.prob.as<LmProblem>();
   unsigned int* ticket = c->d_lm_ticket.as<unsigned int>();
 
   CU(cudaEventRecord(c->ev[3], c->stream));
@@ -1438,11 +1465,12 @@ static int solve_lm(mvicp_ctx* c, bool per_component, const char* fn, int32_t pa
   c->stats.kernel_launches += 1;
   const int64_t max_evals = (int64_t)opt.max_num_iterations + 2;   // per problem, so for the loop as well (no int overflow at INT32_MAX)
   const bool use_p2p = c->comm && c->world > 1 && c->p2p_ok && E <= mvicp_ctx::X_ECAP;
-  const DoneGate gate{&dS[0].done, c->lm_edge_prob, (int32_t)(sizeof(LmState) / sizeof(int))};
+  const DoneGate gate{&dS[0].done, c->lm.edge_prob, (int32_t)(sizeof(LmState) / sizeof(int))};
   const int rob = robust ? 1 : 0;
+  const EvalArgs ea = lm_eval_args(c);
   auto eval = [&]() {
-    if (general) { if (c->f32) launch_eval_general<true>(c, param, cost, rob, gate); else launch_eval_general<false>(c, param, cost, rob, gate); }
-    else if (c->f32) launch_eval<true>(c, cost, rob, gate); else launch_eval<false>(c, cost, rob, gate);
+    if (general) { if (c->f32) launch_eval_general<true>(c, ea, param, cost, rob, gate); else launch_eval_general<false>(c, ea, param, cost, rob, gate); }
+    else if (c->f32) launch_eval<true>(c, ea, cost, rob, gate); else launch_eval<false>(c, ea, cost, rob, gate);
   };
   auto step = [&](size_t dyn) -> int {
     // sharded: pair matrices go straight into every peer's exchange buffer (double-buffered by iteration parity)
@@ -1475,7 +1503,7 @@ static int solve_lm(mvicp_ctx* c, bool per_component, const char* fn, int32_t pa
     c->stats.kernel_launches += (c->n_eval_tiles ? 1 : 0) + 2;
     return MVICP_OK;
   };
-  RET(run_steps(c, lm_step_kernel, c->lm_dyn, max_evals, "LM", w.seq, eval, step));
+  RET(run_steps(c, lm_step_kernel, c->lm.dyn, max_evals, "LM", w.seq, eval, step));
   // sharded runs: every rank holds bit-identical poses (the same lm_step_kernel ran on bit-identical pair matrices), so
   // no pose exchange is needed; the NCCL-only mode still all-gathers the owners' copies (6-dof poses per outer iteration,
   // as the north-star words it) -- a few small copies that change nothing.
@@ -1529,6 +1557,167 @@ int mvicp_get_components(mvicp_ctx* c, int32_t* n_components, int32_t* component
 int mvicp_optimize_components(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt_in,
                               mvicp_lm_summary* summaries) {
   return solve_lm(c, true, "mvicp_optimize_components", param, cost, robust, opt_in, summaries);
+}
+
+// ---- pose covariances (covariance.cuh, DESIGN.md section 6j) ---------------------------------------------------------------
+// The problem of mvicp_optimize (frame 0 and the flagged frames fixed), split into its connected components as
+// mvicp_optimize_components splits it, but without fixing anything: a component without a fixed frame is singular (its gauge is
+// free) and is not factored.  One evaluation at the current poses with the solve's kernels, tile length and eval path, on
+// buffers of this call's own; then cov_factor_kernel per problem and cov_solve_kernel per (problem, frame whose columns some pair
+// needs); the pairs are read out on the host from one copy.  The block of (a, b) always comes from the columns of the one of the
+// two frames with the higher local column, so (b, a) is its exact transpose and no block depends on the other pairs.
+int mvicp_covariance(mvicp_ctx* c, int32_t param, int32_t cost, int32_t robust, int32_t n_pairs, const int32_t* frame_a,
+                     const int32_t* frame_b, double* cov36, int32_t* status) {
+  const char* fn = "mvicp_covariance";
+  if (!c) return fail(MVICP_ERR_INVALID, "%s: null context", fn);
+  if (param < 0 || param > 2 || cost < 0 || cost > 2) return fail(MVICP_ERR_INVALID, "%s: bad param/cost", fn);
+  if (n_pairs < 0 || (n_pairs > 0 && (!frame_a || !frame_b || !cov36))) return fail(MVICP_ERR_INVALID, "%s: bad pair arrays", fn);
+  if (!c->M || !c->E) return fail(MVICP_ERR_STATE, "%s: frames and graph must be set first", fn);
+  if (c->world > 1) return fail(MVICP_ERR_STATE, "%s: the covariance runs on one GPU; this context is sharded", fn);
+  const int M = c->M, E = c->E;
+  for (int k = 0; k < n_pairs; ++k)
+    if (frame_a[k] < 0 || frame_a[k] >= M || frame_b[k] < 0 || frame_b[k] >= M)
+      return fail(MVICP_ERR_INVALID, "%s: pair %d (%d, %d): frame outside [0, %d)", fn, k, frame_a[k], frame_b[k], M);
+  if (cost != COST_P2P && !c->have_normals) return fail(MVICP_ERR_INVALID, "point-to-plane needs normals for every frame");
+  if (!n_pairs) return MVICP_OK;
+  CU(cudaSetDevice(c->device));
+  std::vector<uint8_t> fixed(c->fixed);
+  fixed[0] = 1;   // as mvicp_optimize fixes it (icp-ceres.cpp:242-244)
+  std::vector<int32_t> comp;
+  const int K = graph_components(c, comp);
+  std::vector<std::vector<int32_t>> fr(K), ed(K);
+  std::vector<uint8_t> anchored(K, 0);
+  for (int f = 0; f < M; ++f) { fr[comp[f]].push_back(f); if (fixed[f]) anchored[comp[f]] = 1; }
+  for (int e = 0; e < E; ++e) ed[comp[c->h_edges[e].src]].push_back(e);
+  std::vector<int32_t> col(M, -1), prob_of(K, -1), ns;
+  std::vector<std::vector<int32_t>> pf, pe;
+  for (int k = 0; k < K; ++k) {
+    if (!anchored[k]) continue;
+    int n = 0;
+    for (int f : fr[k]) if (!fixed[f]) { col[f] = n; n += 6; }
+    if (!n) continue;
+    prob_of[k] = (int32_t)pf.size(); ns.push_back(n);
+    pf.push_back(std::move(fr[k])); pe.push_back(std::move(ed[k]));
+  }
+  const int P = (int)pf.size();
+  // classify the pairs; the ones that need C name the frame whose columns hold their block
+  std::vector<int32_t> st(n_pairs), hi_of(n_pairs, -1), job_of(M, -1);
+  std::vector<CovJob> jobs;
+  int64_t out_len = 0;
+  int n_max = 0;
+  for (int k = 0; k < n_pairs; ++k) {
+    const int a = frame_a[k], b = frame_b[k];
+    if (fixed[a] || fixed[b]) { st[k] = MVICP_COV_FIXED; continue; }
+    if (comp[a] != comp[b]) { st[k] = MVICP_COV_INDEPENDENT; continue; }
+    const int q = prob_of[comp[a]];
+    if (q < 0) { st[k] = MVICP_COV_SINGULAR; continue; }
+    st[k] = MVICP_COV_OK;
+    const int hi = col[a] >= col[b] ? a : b;
+    hi_of[k] = hi;
+    if (job_of[hi] < 0) {
+      job_of[hi] = (int32_t)jobs.size();
+      jobs.push_back(CovJob{q, col[hi], out_len});
+      out_len += 6 * (int64_t)ns[q]; n_max = std::max(n_max, ns[q]);
+    }
+  }
+  std::vector<int32_t> pstat(P, MVICP_COV_OK);
+  std::vector<double> hout(out_len);
+  if (!jobs.empty()) {
+    // layout of the problems: cached, as the solves cache theirs
+    std::vector<uint8_t> key(fixed); key.push_back((uint8_t)(c->graph_gen & 0xff)); key.push_back((uint8_t)((c->graph_gen >> 8) & 0xff));
+    if (key != c->cov.key) {
+      std::vector<uint8_t> active(E);
+      for (int e = 0; e < E; ++e) active[e] = !fixed[c->h_edges[e].src];
+      RET(upload_problems(c, c->cov, col, pf, pe, active, key));
+    }
+    // the streaming tiles mvicp_optimize lays out on one GPU once frame 0 is fixed (layout_work)
+    int64_t active_slots = 0;
+    for (int e = 0; e < E; ++e) if (!fixed[c->h_edges[e].src]) active_slots += c->h_edges[e].n_src;
+    const int tl = eval_tile_len_of(active_slots);
+    std::vector<Tile> et; std::vector<int32_t> etb(E + 1, 0);
+    for (int e = 0; e < E; ++e) {
+      etb[e] = (int32_t)et.size();
+      if (fixed[c->h_edges[e].src]) continue;
+      for (int s = 0; s < c->h_edges[e].n_src; s += tl) et.push_back(Tile{e, s});
+    }
+    etb[E] = (int32_t)et.size();
+    const int nt = (int)et.size();
+    std::vector<LmState> hs(P + 1);
+    std::memset(hs.data(), 0, sizeof(LmState) * (P + 1));
+    for (int q = 0; q <= P; ++q) {
+      LmState& s = hs[q];
+      mvicp_default_lm_options(&s.opt);
+      s.param = param; s.cost_kind = cost; s.robust = robust ? 1 : 0; s.G = ambient_size(param);
+      if (q == P) { s.M = M; s.E = E; continue; }
+      s.M = (int32_t)pf[q].size(); s.E = (int32_t)pe[q].size(); s.n = ns[q]; s.F = s.n / 6;
+    }
+    const bool general = poses_nonrigid(c->h_poses.data(), M) && param != PARAM_AA;   // the solve's rule
+    RET(c->d_cov_x.reserve(sizeof(double) * 7 * M)); RET(c->d_cov_cand.reserve(sizeof(double) * 7 * M));
+    RET(c->d_cov_Rt.reserve(sizeof(Rt) * M)); RET(c->d_cov_K.reserve(sizeof(double) * 36 * M));
+    if (general) RET(c->d_cov_gen.reserve(sizeof(FrameGen) * M));
+    RET(c->d_cov_partial.reserve(sizeof(double) * (general ? GBLK : NBLK) * std::max(1, nt)));
+    RET(c->d_cov_eout.reserve(sizeof(double) * EOUT * E));
+    RET(c->d_cov_tiles.reserve(sizeof(Tile) * std::max(1, nt))); RET(c->d_cov_etb.reserve(sizeof(int32_t) * (E + 1)));
+    RET(c->d_cov_status.reserve(sizeof(int32_t) * P)); RET(c->d_cov_jobs.reserve(sizeof(CovJob) * jobs.size()));
+    RET(c->d_cov_out.reserve(sizeof(double) * out_len));
+    LmState* dS = c->cov.state.as<LmState>();
+    CU(cudaMemcpyAsync(dS, hs.data(), sizeof(LmState) * (P + 1), cudaMemcpyHostToDevice, c->stream));
+    if (nt) CU(cudaMemcpyAsync(c->d_cov_tiles.p, et.data(), sizeof(Tile) * nt, cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(c->d_cov_etb.p, etb.data(), sizeof(int32_t) * (E + 1), cudaMemcpyHostToDevice, c->stream));
+    CU(cudaMemcpyAsync(c->d_cov_jobs.p, jobs.data(), sizeof(CovJob) * jobs.size(), cudaMemcpyHostToDevice, c->stream));
+    LmWork w{};
+    w.S = dS + P; w.x = c->d_cov_x.as<double>(); w.cand = c->d_cov_cand.as<double>(); w.Rt_eval = c->d_cov_Rt.as<Rt>();
+    w.K_eval = c->d_cov_K.as<double>(); w.G_eval = general ? c->d_cov_gen.as<FrameGen>() : nullptr; w.poses16 = c->d_poses.as<double>();
+    lm_init_kernel<<<(M + 63) / 64, 64, 0, c->stream>>>(w);
+    const DoneGate gate{&dS[0].done, c->cov.edge_prob, (int32_t)(sizeof(LmState) / sizeof(int))};
+    const EvalArgs ea{c->d_cov_tiles.as<Tile>(), nt, tl, c->d_cov_Rt.as<Rt>(), c->d_cov_gen.as<FrameGen>(), c->d_cov_partial.as<double>()};
+    const int rob = robust ? 1 : 0;
+    if (general) { if (c->f32) launch_eval_general<true>(c, ea, param, cost, rob, gate); else launch_eval_general<false>(c, ea, param, cost, rob, gate); }
+    else if (c->f32) launch_eval<true>(c, ea, cost, rob, gate); else launch_eval<false>(c, ea, cost, rob, gate);
+    PeerTable pt; std::memset(&pt, 0, sizeof pt); pt.world = 1; pt.rank = 0;
+    double* eout = c->d_cov_eout.as<double>();
+    if (general)
+      lm_edge_general_kernel<<<E, EDGE_THREADS, 0, c->stream>>>(c->d_edges.as<EdgeDev>(), c->d_cov_etb.as<int32_t>(),
+                                                                c->d_cov_partial.as<double>(), eout, gate, pt, 0, nullptr);
+    else
+      lm_edge_kernel<<<E, EDGE_THREADS, 0, c->stream>>>(c->d_edges.as<EdgeDev>(), c->d_cov_etb.as<int32_t>(), c->d_cov_partial.as<double>(),
+                                                        cost == COST_P2PLANE ? NBLK_PLANE : NBLK, c->d_cov_Rt.as<Rt>(), c->d_cov_K.as<double>(),
+                                                        eout, gate, pt, 0, nullptr);
+    const LmProblem* probs = c->cov.prob.as<LmProblem>();
+    int32_t* dstat = c->d_cov_status.as<int32_t>();
+    CU(cudaFuncSetAttribute(cov_factor_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    cov_factor_kernel<<<P, STEP_THREADS, c->cov.dyn, c->stream>>>(probs, eout, dstat);
+    const size_t vec = sizeof(double) * 6 * (size_t)n_max;
+    const int vec_in_smem = vec <= 220 * 1024 ? 1 : 0;
+    if (vec_in_smem) CU(cudaFuncSetAttribute(cov_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 220 * 1024));
+    cov_solve_kernel<<<(int)jobs.size(), COV_SOLVE_THREADS, vec_in_smem ? vec : 0, c->stream>>>(probs, c->d_cov_jobs.as<CovJob>(), dstat,
+                                                                                               c->d_cov_out.as<double>(), vec_in_smem);
+    c->stats.kernel_launches += 4 + (nt ? 1 : 0);
+    CU(cudaMemcpyAsync(pstat.data(), dstat, sizeof(int32_t) * P, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaMemcpyAsync(hout.data(), c->d_cov_out.p, sizeof(double) * out_len, cudaMemcpyDeviceToHost, c->stream));
+    CU(cudaStreamSynchronize(c->stream));
+    CU(cudaGetLastError());
+  }
+  // the blocks: Cov(a, b)[i][j] = C[col a + i][col b + j], read from the columns of hi = the frame with the higher column
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  for (int k = 0; k < n_pairs; ++k) {
+    double* o = cov36 + 36 * (size_t)k;
+    const int a = frame_a[k], b = frame_b[k], hi = hi_of[k];
+    if (st[k] == MVICP_COV_OK && pstat[prob_of[comp[a]]] != MVICP_COV_OK) st[k] = MVICP_COV_SINGULAR;
+    if (status) status[k] = st[k];
+    if (st[k] == MVICP_COV_FIXED || st[k] == MVICP_COV_INDEPENDENT) { for (int i = 0; i < 36; ++i) o[i] = 0.0; continue; }
+    if (st[k] == MVICP_COV_SINGULAR) { for (int i = 0; i < 36; ++i) o[i] = nan; continue; }
+    const CovJob& jb = jobs[job_of[hi]];
+    const int n = ns[jb.prob];
+    const double* base = hout.data() + jb.at;   // column col[hi] + j at base[j n ..]
+    for (int i = 0; i < 6; ++i)
+      for (int j = 0; j < 6; ++j) {
+        if (a == b) o[6 * i + j] = 0.5 * (base[(size_t)j * n + col[a] + i] + base[(size_t)i * n + col[a] + j]);   // exactly symmetric
+        else if (b == hi) o[6 * i + j] = base[(size_t)j * n + col[a] + i];
+        else o[6 * i + j] = base[(size_t)i * n + col[b] + j];
+      }
+  }
+  return MVICP_OK;
 }
 
 int mvicp_icp_round(mvicp_ctx* c, float thresh, int32_t param, int32_t cost, int32_t robust, const mvicp_lm_options* opt, mvicp_lm_summary* summary) {
@@ -1649,7 +1838,7 @@ static int solve_g2o(mvicp_ctx* c, bool per_component, const char* fn, int32_t c
   for (int e = 0; e < E; ++e) active[e] = cnt[e] != 0;
   std::vector<uint8_t> key(c->fixed); key.push_back((uint8_t)(c->graph_gen & 0xff)); key.push_back((uint8_t)((c->graph_gen >> 8) & 0xff));
   key.push_back(per_component ? 3 : 2);
-  RET(upload_problems(c, pf, pe, active, key));
+  RET(upload_problems(c, c->lm, c->h_col, pf, pe, active, key));
   const int64_t cap = std::max<int64_t>(G2O_TRACE_MIN, G2O_TRACE_CAP / P);
   RET(c->d_g2o_state.reserve(sizeof(G2oState) * P)); RET(c->d_g2o_prob.reserve(sizeof(G2oProblem) * P));
   RET(c->d_g2o_x.reserve(sizeof(Rt) * M)); RET(c->d_g2o_ev.reserve(sizeof(Rt) * M)); RET(c->d_g2o_nop.reserve(sizeof(int32_t) * M));
@@ -1665,7 +1854,7 @@ static int solve_g2o(mvicp_ctx* c, bool per_component, const char* fn, int32_t c
     s.max_iter = opt.iterations_per_call; s.max_calls = opt.max_calls;
     s.no_impr_limit = opt.no_improvement_limit; s.max_trials = opt.max_trials; s.ortho_after = opt.orthonormalize_after;
     s.phase = G2O_BUILD; s.trace_cap = (int32_t)cap; s.tau = opt.tau;
-    const LmProblem& lp = c->h_prob[q];
+    const LmProblem& lp = c->lm.h_prob[q];
     probs[q] = G2oProblem{dS + q, lp.frame, lp.edge, lp.lay, lp.H, lp.g, c->d_g2o_chi.as<double>() + row * q,
                           c->d_g2o_trace.as<double>() + 5 * (size_t)cap * q};
   }
@@ -1686,7 +1875,7 @@ static int solve_g2o(mvicp_ctx* c, bool per_component, const char* fn, int32_t c
   const int64_t max_evals = (int64_t)opt.max_calls * opt.iterations_per_call * (opt.max_trials + 1) + 2;   // per problem, so for the loop
   const double eps = opt.information_eps;
   // the joint solve (every edge in problem 0) runs without the edge -> problem lookup and with its own step kernel
-  const G2oGate gate{dS, per_component ? c->lm_edge_prob : nullptr};
+  const G2oGate gate{dS, per_component ? c->lm.edge_prob : nullptr};
   auto eval = [&]() { if (c->f32) launch_g2o_eval<true>(c, cost, nt, gate, eps); else launch_g2o_eval<false>(c, cost, nt, gate, eps); };
   auto step = [&](size_t dyn) -> int {
     g2o_edge_kernel<<<E, EDGE_THREADS, 0, c->stream>>>(c->d_g2o_tile_begin.as<int32_t>(), c->d_partial.as<double>(), gate, c->d_eout.as<double>());
@@ -1695,8 +1884,8 @@ static int solve_g2o(mvicp_ctx* c, bool per_component, const char* fn, int32_t c
     c->stats.kernel_launches += 3;
     return MVICP_OK;
   };
-  if (per_component) RET(run_steps(c, g2o_step_kernel, c->lm_dyn, max_evals, "g2o", w.seq, eval, step));
-  else RET(run_steps(c, g2o_step_one_kernel, c->lm_dyn, max_evals, "g2o", w.seq, eval, step));
+  if (per_component) RET(run_steps(c, g2o_step_kernel, c->lm.dyn, max_evals, "g2o", w.seq, eval, step));
+  else RET(run_steps(c, g2o_step_one_kernel, c->lm.dyn, max_evals, "g2o", w.seq, eval, step));
   RET(read_back_solve(c, st.data(), dS, sizeof(G2oState) * P));
   std::vector<double> chis;
   if (chi2_per_call) {
