@@ -131,8 +131,10 @@ struct mvicp_ctx {
   std::vector<float> h_weight; std::vector<unsigned long long> h_count;
   // LM
   DevBuf d_x, d_cand, d_Rt, d_K, d_eout, d_posegather, d_gen;
-  int lm_blocks_E = 0;         // edges of the LM evaluation d_eout holds; 0: none since the graph was set, or a g2o solve reused it
-  std::vector<uint8_t> lm_blocks_fixed;   // the fixed flags of that solve: the edges of a fixed src read as zeros
+  int lm_blocks_E = 0;         // edges of the evaluation d_eout holds; 0: none since the graph was set, or the last solve failed
+  bool blocks_g2o = false;     // that evaluation is a g2o solve's (g2o_edge_kernel's records), not an LM solve's
+  std::vector<uint8_t> lm_blocks_fixed;   // LM: the fixed flags of that solve: the edges of a fixed src read as zeros
+  std::vector<uint8_t> g2o_blocks_unwritten;   // g2o: the edges no evaluation of that solve wrote (they read as zeros)
   std::vector<int32_t> h_col;
   volatile int32_t* h_flag = nullptr; volatile int32_t* d_flag = nullptr;   // mapped pinned ring written by the step kernels
   uint32_t graph_gen = 0;
@@ -1536,7 +1538,7 @@ static int solve_lm(mvicp_ctx* c, bool per_component, const char* fn, int32_t pa
   if (st[P].nonrigid && !general)   // cannot happen after mvicp_set_poses; guards poses that reached the device another way
     return fail(MVICP_ERR_NONRIGID, "a pose's quaternion is not unit (non-rigid Isometry) but the unit-quaternion LM path was run");
   if (!all_done) return fail(MVICP_ERR_STATE, "LM loop did not terminate within %lld evaluations", (long long)max_evals);
-  c->lm_blocks_E = E; c->lm_blocks_fixed = c->fixed;
+  c->lm_blocks_E = E; c->blocks_g2o = false; c->lm_blocks_fixed = c->fixed;
   return MVICP_OK;
 }
 
@@ -1770,7 +1772,7 @@ static int solve_g2o(mvicp_ctx* c, bool per_component, const char* fn, int32_t c
   mvicp_g2o_options opt; if (opt_in) opt = *opt_in; else mvicp_default_g2o_options(&opt);
   if (opt.iterations_per_call < 1 || opt.max_calls < 1 || opt.max_trials < 1 || opt.no_improvement_limit < 0 || opt.orthonormalize_after < 0)
     return fail(MVICP_ERR_INVALID, "%s: bad options", fn);
-  c->lm_blocks_E = 0;   // the g2o solve writes its own edge blocks into d_eout
+  c->lm_blocks_E = 0;   // until this solve has run: it writes its own edge blocks into d_eout
   CU(cudaSetDevice(c->device));
   const int M = c->M, E = c->E;
   std::vector<int32_t> comp(M, 0);
@@ -1830,8 +1832,15 @@ static int solve_g2o(mvicp_ctx* c, bool per_component, const char* fn, int32_t c
     if (summaries) summaries[k].ended = MVICP_G2O_END_NO_VERTICES;
     if (chi2_per_call) chi2_per_call[row * k] = 0.0;
   };
+  // mvicp_debug_edge_blocks after this solve: the edges of a component without a problem are never evaluated
+  auto readout_after = [&]() {
+    c->g2o_blocks_unwritten.assign(E, 0);
+    for (int e = 0; e < E; ++e) c->g2o_blocks_unwritten[e] = prob_of[comp[c->h_edges[e].src]] < 0;
+    c->lm_blocks_E = E; c->blocks_g2o = true;
+  };
   if (!P) {
     for (int k = 0; k < K; ++k) no_vertices(k);
+    readout_after();
     return MVICP_OK;
   }
   std::vector<uint8_t> active(E);
@@ -1910,6 +1919,7 @@ static int solve_g2o(mvicp_ctx* c, bool per_component, const char* fn, int32_t c
     }
   }
   if (!all_done) return fail(MVICP_ERR_STATE, "g2o solve did not terminate within %lld evaluations", (long long)max_evals);
+  readout_after();
   return MVICP_OK;
 }
 
@@ -2255,7 +2265,7 @@ int mvicp_debug_step_profile(mvicp_ctx* c, long long* out64) {
   CU(cudaMemcpy(out64, c->d_prof.p, sizeof(long long) * 64, cudaMemcpyDeviceToHost));
   return MVICP_OK;
 }
-// development aid: the per-edge output of the last LM evaluation, E x 160 doubles (EOUT), as lm_edge_kernel /
+// development aid: the per-edge output of the last LM (or g2o, below) evaluation, E x 160 doubles (EOUT), as lm_edge_kernel /
 // lm_edge_general_kernel wrote it and gather_blocks / gather_gradient / edge_cost_sum read it.  Edge e's record:
 //   [0, 144)    the 12x12 pair matrix Hp, row-major; rows and columns 0-5 are the src frame's tangent, 6-11 the dst frame's
 //               (lm_step's sub-blocks ss | sk over ks | kk)
@@ -2267,20 +2277,40 @@ int mvicp_debug_step_profile(mvicp_ctx* c, long long* out64) {
 // written, so the readout zeroes every such record itself.  The blocks are those of the LAST evaluation: after
 // mvicp_optimize with max_num_iterations = 0 the start point; after a rejected step the rejected candidate.  The evaluation
 // enqueued behind a finished solve is skipped by its DoneGate and leaves them alone.  In a component solve each edge holds its
-// own problem's last evaluation.  MVICP_ERR_STATE before any LM solve has evaluated since the graph was set, after a g2o
-// solve, after a solve that failed, and in a sharded context.  Launches nothing and changes no state.
+// own problem's last evaluation.
+// After mvicp_optimize_g2o / mvicp_optimize_g2o_components the records are g2o_edge_kernel's, in the same layout: the pair
+// matrix over [src | dst] and the gradient sum J^T Omega e (g2o's b is -g), both in g2o's increment order (tx ty tz qx qy
+// qz); slot 156 the edge's chi2 sum e^T Omega e (no 1/2); 157-159 zero.  Slots 0-155 come from the last build of the edge's
+// problem, slot 156 from its last evaluation, build or trial (a trial writes only slot 156).  An edge out of a fixed frame
+// into a free one is active and reads as its full record; an edge between two fixed frames reads as zeros.  The edges of a
+// component without a g2o problem, and every edge when no problem has a vertex, are never written and read as zeros.
+// MVICP_ERR_STATE before any LM or g2o solve has evaluated since the graph was set, after a solve that failed once it had
+// started, and in a sharded context.  A call refused for its arguments (state, cost, normals, options) touches nothing, so
+// the previous solve's records stay readable after it.  Launches nothing and changes no state.
 int mvicp_debug_edge_blocks(mvicp_ctx* c, double* out, int64_t capacity, int32_t* n_edges) {
   if (!c || !n_edges) return fail(MVICP_ERR_INVALID, "mvicp_debug_edge_blocks: bad arguments");
   if (c->world > 1) return fail(MVICP_ERR_STATE, "mvicp_debug_edge_blocks: the context is sharded");
-  if (!c->lm_blocks_E || c->lm_blocks_E != c->E) return fail(MVICP_ERR_STATE, "mvicp_debug_edge_blocks: no completed LM solve since the graph was set");
+  if (!c->lm_blocks_E || c->lm_blocks_E != c->E) return fail(MVICP_ERR_STATE, "mvicp_debug_edge_blocks: no completed LM or g2o solve since the graph was set");
   *n_edges = c->E;
   if (!out) return MVICP_OK;
   if (capacity < (int64_t)EOUT * c->E) return fail(MVICP_ERR_INVALID, "mvicp_debug_edge_blocks: capacity %lld < %lld", (long long)capacity, (long long)EOUT * c->E);
   CU(cudaSetDevice(c->device));
   CU(cudaStreamSynchronize(c->stream));
-  CU(cudaMemcpy(out, c->d_eout.p, sizeof(double) * EOUT * c->E, cudaMemcpyDeviceToHost));
-  for (int e = 0; e < c->E; ++e)
-    if (c->lm_blocks_fixed[c->h_edges[e].src]) std::memset(out + (size_t)EOUT * e, 0, sizeof(double) * EOUT);
+  const size_t rec = sizeof(double) * EOUT;
+  if (!c->blocks_g2o) {
+    CU(cudaMemcpy(out, c->d_eout.p, rec * c->E, cudaMemcpyDeviceToHost));
+    for (int e = 0; e < c->E; ++e)
+      if (c->lm_blocks_fixed[c->h_edges[e].src]) std::memset(out + (size_t)EOUT * e, 0, rec);
+    return MVICP_OK;
+  }
+  bool any = false;   // a g2o solve without a vertex evaluated nothing (and may have found no d_eout)
+  for (int e = 0; e < c->E; ++e) any = any || !c->g2o_blocks_unwritten[e];
+  if (any) CU(cudaMemcpy(out, c->d_eout.p, rec * c->E, cudaMemcpyDeviceToHost));
+  for (int e = 0; e < c->E; ++e) {
+    double* o = out + (size_t)EOUT * e;
+    if (c->g2o_blocks_unwritten[e]) std::memset(o, 0, rec);
+    else o[157] = o[158] = o[159] = 0.0;   // g2o_edge_kernel writes slots 0-156 only
+  }
   return MVICP_OK;
 }
 int mvicp_get_stream(mvicp_ctx* c, void** stream) { if (!c || !stream) return fail(MVICP_ERR_INVALID, "bad arguments"); *stream = (void*)c->stream; return MVICP_OK; }
